@@ -1,9 +1,9 @@
-"""aesara_b200 — a Blackwell (sm_100a) execution backend behind Aesara's Linker.
+"""aesara_b200 — a Hopper (H100, sm_90a) execution backend behind Aesara's Linker.
 
 ``import aesara_b200`` registers linker ``"b200"`` and mode ``"B200"`` with the
 reference front-end when it is importable (``aesara_b200.linker``).  The device
 runtime itself (``aesara_b200.runtime``, ``aesara_b200.ir``) has no Aesara
-dependency: lowered programs run wherever ``libaesara_b200.so`` and a B200 are.
+dependency: lowered programs run wherever ``libaesara_b200.so`` and an H100 are.
 """
 
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-"""Build ``libaesara_b200.so`` in-tree with nvcc for sm_100a.
+"""Build ``libaesara_b200.so`` in-tree with nvcc for sm_90a (H100).
 
 ``python -m aesara_b200.build`` (or ``__graft_entry__.build()``).  nvcc
 cross-compiles without a GPU; the resulting ``.so`` is git-ignored but travels
@@ -19,7 +19,7 @@ LIBDIR = os.path.join(PKG, "lib")
 LIBNAME = "libaesara_b200.so"
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall",
           "-Xcompiler", "-Wno-unused-function"]
 

@@ -5,7 +5,7 @@
 // the same (shape, strides, reduce-mask) description is canonicalised — size-1
 // dims dropped, neighbours of equal kind merged — and mapped to one of two
 // access patterns, with the reduced range split across CTAs when there are too
-// few outputs to fill 148 SMs (two deterministic stages through `workspace`).
+// few outputs to fill the 132 SMs (two deterministic stages through `workspace`).
 #include <algorithm>
 #include <vector>
 
@@ -38,7 +38,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
   }
   return n;
 }

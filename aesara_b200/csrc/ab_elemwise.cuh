@@ -209,7 +209,7 @@ ab_ew_rows(const __grid_constant__ AbEwParams p) {
 // threads, 16 elements per thread: 16 independent loads per input in flight per thread.
 #define AB_TILE 64
 #ifndef AB_TILE_BAND
-#define AB_TILE_BAND 1  // measured: bands of 2-32 tile rows are 10 % slower (profiles/r02_ew_transposed_tile64.json)
+#define AB_TILE_BAND 1  // tile rows per CTA
 #endif
 __host__ __device__ constexpr int ab_max_input_size() {
   int m = 1;

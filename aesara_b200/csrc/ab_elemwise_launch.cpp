@@ -45,7 +45,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
   }
   return n;
 }

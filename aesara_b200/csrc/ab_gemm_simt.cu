@@ -1,9 +1,9 @@
 // ab_gemm_simt.cu — C <- beta*C + alpha*A@B on the FP32/FP64 CUDA-core pipes.
 //
 // This is the float64 path of Gemm/Dot22 (aesara/tensor/blas.py:872/:1659 accept
-// float32 and float64 only, :613-629; tcgen05 has no f64 kind) and the path for
+// float32 and float64 only, :613-629; the tensor-core path is float32 only) and the path for
 // problems too small or too oddly strided for the TMA-fed tensor-core kernel in
-// ab_gemm_tcgen05.cu.  Classic shared-memory tiling: 64x64 output tile per CTA,
+// ab_gemm_tc.cu.  Classic shared-memory tiling: 64x64 output tile per CTA,
 // K stepped by 16, each of the 256 threads owns a 4x4 register micro-tile.
 // Arbitrary element strides for A, B, C (the eight transposed/strided cases of
 // blas.py:765-776 need no copies here).

@@ -103,7 +103,7 @@ __global__ void clear_flag_kernel(int* f) { *f = 0; }
 
 unsigned grid_for(long long total) {
   long long b = (total + kThreads - 1) / kThreads;
-  return (unsigned)std::max<long long>(1, std::min<long long>(b, 148LL * 32));
+  return (unsigned)std::max<long long>(1, std::min<long long>(b, 132LL * 32));
 }
 
 template <typename IDX>

@@ -62,7 +62,7 @@ using namespace ab;
 
 extern "C" {
 
-const char* ab_version(void) { return "aesara_b200 0.1 (sm_100a)"; }
+const char* ab_version(void) { return "aesara_b200 0.1 (sm_90a)"; }
 
 const char* ab_last_error(void) { return last_error().c_str(); }
 
@@ -162,7 +162,7 @@ int ab_nvrtc_compile(const char* src, const char* name, const char* const* extra
   nvrtcProgram prog;
   nvrtcResult r = nvrtcCreateProgram(&prog, src, name ? name : "ab_module.cu", 0, nullptr, nullptr);
   if (r != NVRTC_SUCCESS) return fail(AB_ERR_NVRTC, "nvrtcCreateProgram: %s", nvrtcGetErrorString(r));
-  std::vector<const char*> opts = {"--gpu-architecture=sm_100a", "--std=c++17", "-lineinfo",
+  std::vector<const char*> opts = {"--gpu-architecture=sm_90a", "--std=c++17", "-lineinfo",
                                    "-default-device"};
   for (int i = 0; i < n_extra_opts; ++i) opts.push_back(extra_opts[i]);
   r = nvrtcCompileProgram(prog, (int)opts.size(), opts.data());

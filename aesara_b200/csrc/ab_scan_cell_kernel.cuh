@@ -14,48 +14,27 @@
 // AB_CELL_EVAL(G, P, O): float G[GATES] pre-activations, float P[STATES] previous states ->
 // float O[STATES] new states, for one (row, hidden unit).
 //
-//   * persistent cooperative grid, one CTA (or CTA pair, cta_group::2) per SM; every step the
-//     [B, G*H] pre-activation is produced as 128/256 x (G*64) tcgen05 tiles (3xTF32, fp32-
-//     faithful like ab_gemm) whose columns are the G gates of 64 hidden units (U is packed
-//     once with its columns gate-interleaved);
-//   * the cell is the tile's epilogue: accumulators come out of TMEM, x_t and the previous
+//   * persistent cooperative grid, one CTA per SM; every step the [B, G*H] pre-activation is
+//     produced as 64 x (G*64) wgmma tiles (3xTF32, fp32-faithful like ab_gemm) whose columns
+//     are the G gates of 64 hidden units (U is packed once with its columns gate-interleaved);
+//   * the cell is the tile's epilogue, run in the accumulator registers: x_t and the previous
 //     states are read once, the new states go to the Scan's circular output buffers and the
 //     state that feeds the Gemm is ALSO written as the hi/lo TF32 planes the next step's TMA
-//     loads; K is accumulated in 256-element segments (fresh TMEM accumulator each, summed in
-//     FP32 registers) because the tensor core's own accumulate truncates;
+//     loads; K is accumulated in 256-element segments (fresh register accumulator each, summed
+//     in FP32 with round-to-nearest) because the tensor core's own accumulate truncates;
 //   * no barrier between steps: batch rows are independent, so a tile of step t+1 waits only
-//     for the step-t tiles of ITS row block (per-row-block counters: bar.sync of the epilogue
+//     for the step-t tiles of ITS row block (per-row-block counters: bar.sync of the consumer
 //     warps, __threadfence, atomicAdd; acquire load + fence.proxy.async on the producer side);
-//   * three warpgroups: {TMA producer, MMA issuer, two idle warps} give most of their registers
-//     back (setmaxnreg.dec) and the eight epilogue warps take them (setmaxnreg.inc): the G x 32
-//     accumulator registers plus the cell's temporaries fit without spills (the 320-thread
-//     layout of round 1 was capped at 168 registers and spilled 180-288 bytes).
+//   * three warpgroups: {TMA producer, three idle warps} give most of their registers back
+//     (setmaxnreg.dec) and the two consumer warpgroups take them (setmaxnreg.inc); consumer
+//     warpgroup s issues the wgmma of hidden units [32 s, 32 s + 32) of the tile (G products
+//     of N = 32 per K step) and evaluates the cell on them: G x 16 accumulator registers plus
+//     as many for the running sum.
 #pragma once
 
 constexpr int kCellThreads = 384;
 constexpr int kCellEpiThreads = 256;
-// Each epilogue warp owns 4 KB of shared memory behind the operand ring (a 32 x 32 float32
-// block, 16-byte groups XOR-swizzled with the row as in the GEMM epilogue regions): x_t is read
-// and the new states / operand planes are written in a COALESCED layout (eight lanes per
-// 128-byte line) and turned to / from the accumulator layout (lane = row) through it.  In the
-// accumulator layout every 128-bit access touches 32 different lines: of the 80 such accesses
-// per thread and LSTM tile (32 x_t, 16 previous state, 16 ring, 16 plane) 64 are coalesced now.
-constexpr int kCellStageBytesPerWarp = 32 * 32 * 4;
-constexpr int kCellStageBytes = (kCellEpiThreads / 32) * kCellStageBytesPerWarp;
-__device__ __forceinline__ uint32_t cell_st_off(int r, int g) { return (uint32_t)(r * 32 + ((g ^ (r & 7)) << 2)) * 4u; }
-// coalesced layout (v[4 i .. 4 i + 3] = row 4 i + lane / 8, columns 4 (lane % 8) ..) -> lane = row
-__device__ __forceinline__ void cell_to_rows(float (&v)[32], uint32_t stg, int lane) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    sts128(stg + cell_st_off(4 * i + (lane >> 3), lane & 7), v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-  __syncwarp();
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const float4 q = lds128(stg + cell_st_off(lane, g));
-    v[4 * g] = q.x; v[4 * g + 1] = q.y; v[4 * g + 2] = q.z; v[4 * g + 3] = q.w;
-  }
-  __syncwarp();
-}
+constexpr int CELL_BLOCK_M = 64;                         // batch rows per tile
 constexpr int CELL_UNITS = 64;                           // hidden units per tile
 constexpr int CELL_TILE_N = AB_CELL_GATES * CELL_UNITS;  // accumulator columns
 constexpr int CELL_KB = 32;                              // K elements (tf32) per 128-byte smem row
@@ -72,20 +51,10 @@ struct CellParams {
   unsigned int* row_done;    // per row block: tiles completed so far, all steps (zero-initialised)
   int stages;
   int a_tile_bytes, b_tile_bytes;
-  uint32_t idesc;
 };
 
 __device__ __forceinline__ float sigmoidf_ref(float v) { return 1.0f / (1.0f + expf(-v)); }
 
-// acc (+)= 32 accumulator columns of this thread's TMEM lane (round-to-nearest adds)
-__device__ __forceinline__ void cell_fold32(float (&acc)[32], uint32_t taddr) {
-  uint32_t r[32];
-  tmem_ld_32x32b_x32(taddr, r);
-#pragma unroll
-  for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r[j]);
-}
-
-template <int CTAS>
 __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const CUtensorMap& map_h01,
                                                const CUtensorMap& map_h10, const CUtensorMap& map_h11,
                                                const CUtensorMap& map_u0, const CUtensorMap& map_u1,
@@ -95,81 +64,44 @@ __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const
                                              ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[8];
   __shared__ __align__(8) uint64_t empty_bar[8];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_slot;
 
-  constexpr bool TWO = CTAS == 2;
-  constexpr int TILE_M = CTAS * BLOCK_M;
   constexpr int G = AB_CELL_GATES, S = AB_CELL_STATES;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = TWO ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  const long long group_id = blockIdx.x / CTAS, n_groups = gridDim.x / CTAS;
   const int stage_bytes = 2 * (p.a_tile_bytes + p.b_tile_bytes);  // hi + lo of A and B
   const int num_k_blocks = (int)((p.H + CELL_KB - 1) / CELL_KB);
   const long long tiles_n = p.H / CELL_UNITS;
-  const long long num_tiles = ((p.B + TILE_M - 1) / TILE_M) * tiles_n;
-  // two accumulator stages; the allocation is a power of two >= 32 columns
-  constexpr uint32_t tmem_cols = (2 * CELL_TILE_N <= 128) ? 128u : ((2 * CELL_TILE_N <= 256) ? 256u : 512u);
+  const long long num_tiles = ((p.B + CELL_BLOCK_M - 1) / CELL_BLOCK_M) * tiles_n;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full_bar[s], 1);
-      mbar_init(&tmem_empty_bar[s], CTAS * kCellEpiThreads);  // every epilogue thread of the group
+      mbar_init(&empty_bar[s], kCellEpiThreads / 32);  // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    if (TWO) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       smem_u32(&tmem_base_slot)),
-                   "r"(tmem_cols)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                       smem_u32(&tmem_base_slot)),
-                   "r"(tmem_cols)
-                   : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  if (TWO) cluster_sync_all();  // both CTAs' barriers exist before any remote signal
-  tcgen05_fence_after();
-  const uint32_t tmem_base = tmem_base_slot;
 
   // Register budget per SM sub-partition (3 warps each): 56 + 2 x 224 <= 512.  Each role runs
   // its whole T-step loop inside its own branch: ptxas allocates the code that follows a
   // setmaxnreg up to that count only while the branches do not merge again.
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    // pipeline state persists across tiles and steps
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t it = 0;
     if (warp == 0 && elect_one()) {
-      // ================= TMA producer (one per CTA) =================
+      // ================= TMA producer =================
+      int stage = 0;
+      uint32_t phase = 0;
       for (long long t = 0; t < p.T; ++t) {
         const int set = (int)(t & 1);  // planes read this step; the other set is written
-        {
         const CUtensorMap* mh0 = set ? &map_h10 : &map_h00;
         const CUtensorMap* mh1 = set ? &map_h11 : &map_h01;
-        for (long long tile = group_id; tile < num_tiles; tile += n_groups) {
-          const int m0 = (int)((tile / tiles_n) * TILE_M) + (int)rank * BLOCK_M;
-          const int n0 = (int)((tile % tiles_n) * CELL_TILE_N) + (int)rank * (CELL_TILE_N / 2);
+        for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+          const int m0 = (int)((tile / tiles_n) * CELL_BLOCK_M);
+          const int n0 = (int)((tile % tiles_n) * CELL_TILE_N);
           if (t > 0) {
-            // rows of s_hs[t-1] for this row block exist once all of its step t-1 tiles are
-            // counted (tiles_n tiles x CTAS signalling CTAs per step)
-            const unsigned int target = (unsigned int)(t * tiles_n * CTAS);
+            // rows of s_hs[t-1] for this row block exist once all of its step t-1 tiles are counted
+            const unsigned int target = (unsigned int)(t * tiles_n);
             const unsigned int* flag = p.row_done + tile / tiles_n;
             unsigned int seen;
             do {
@@ -181,77 +113,26 @@ __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const
           for (int kb = 0; kb < num_k_blocks; ++kb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sbase = smem + (size_t)stage * stage_bytes;
-            if (leader) mbar_expect_tx(&full_bar[stage], (uint32_t)(CTAS * stage_bytes));
+            mbar_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
             const int kc = kb * CELL_KB;
-            uint8_t* a_hi = sbase;
-            uint8_t* a_lo = sbase + p.a_tile_bytes;
             uint8_t* b_hi = sbase + 2 * p.a_tile_bytes;
-            uint8_t* b_lo = b_hi + p.b_tile_bytes;
-            if (TWO) {
-              tma_load_2d_2sm(a_hi, mh0, &full_bar[stage], kc, m0);
-              tma_load_2d_2sm(a_lo, mh1, &full_bar[stage], kc, m0);
-              tma_load_2d_2sm(b_hi, &map_u0, &full_bar[stage], kc, n0);
-              tma_load_2d_2sm(b_lo, &map_u1, &full_bar[stage], kc, n0);
-            } else {
-              tma_load_2d(a_hi, mh0, &full_bar[stage], kc, m0);
-              tma_load_2d(a_lo, mh1, &full_bar[stage], kc, m0);
-              tma_load_2d(b_hi, &map_u0, &full_bar[stage], kc, n0);
-              tma_load_2d(b_lo, &map_u1, &full_bar[stage], kc, n0);
-            }
+            tma_load_2d(sbase, mh0, &full_bar[stage], kc, m0);
+            tma_load_2d(sbase + p.a_tile_bytes, mh1, &full_bar[stage], kc, m0);
+            tma_load_2d(b_hi, &map_u0, &full_bar[stage], kc, n0);
+            tma_load_2d(b_hi + p.b_tile_bytes, &map_u1, &full_bar[stage], kc, n0);
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
-          }
-        }
-        }
-      }
-    } else if (warp == 1 && leader && elect_one()) {
-      // ================= MMA issuer (the leader CTA of a pair) =================
-      for (long long t = 0; t < p.T; ++t) {
-        for (long long tile = group_id; tile < num_tiles; tile += n_groups) {
-          for (int kb0 = 0; kb0 < num_k_blocks; kb0 += CELL_SEG_KB, ++it) {
-            const int kb1 = min(kb0 + CELL_SEG_KB, num_k_blocks);
-            const uint32_t as = it & 1u, aphase = (it >> 1) & 1u;
-            mbar_wait(&tmem_empty_bar[as], aphase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t d_tmem = tmem_base + as * CELL_TILE_N;
-            for (int kb = kb0; kb < kb1; ++kb) {
-              mbar_wait(&full_bar[stage], phase);
-              tcgen05_fence_after();
-              const uint32_t sbase = smem_u32(smem + (size_t)stage * stage_bytes);
-              const uint32_t a_hi = sbase, a_lo = sbase + p.a_tile_bytes;
-              const uint32_t b_hi = sbase + 2 * p.a_tile_bytes, b_lo = b_hi + p.b_tile_bytes;
-#pragma unroll
-              for (int k = 0; k < SW_BYTES / 32; ++k) {
-                const uint32_t ko = k * 32;
-                const uint32_t acc = (kb > kb0 || k > 0) ? 1u : 0u;
-                if (TWO) {
-                  umma_2sm<0>(d_tmem, make_smem_desc(a_lo + ko, 16), make_smem_desc(b_hi + ko, 16), p.idesc, acc);
-                  umma_2sm<0>(d_tmem, make_smem_desc(a_hi + ko, 16), make_smem_desc(b_lo + ko, 16), p.idesc, 1u);
-                  umma_2sm<0>(d_tmem, make_smem_desc(a_hi + ko, 16), make_smem_desc(b_hi + ko, 16), p.idesc, 1u);
-                } else {
-                  umma<0>(d_tmem, make_smem_desc(a_lo + ko, 16), make_smem_desc(b_hi + ko, 16), p.idesc, acc);
-                  umma<0>(d_tmem, make_smem_desc(a_hi + ko, 16), make_smem_desc(b_lo + ko, 16), p.idesc, 1u);
-                  umma<0>(d_tmem, make_smem_desc(a_hi + ko, 16), make_smem_desc(b_hi + ko, 16), p.idesc, 1u);
-                }
-              }
-              if (TWO) tcgen05_commit_2sm(&empty_bar[stage]);
-              else tcgen05_commit(&empty_bar[stage]);
-              if (++stage == p.stages) { stage = 0; phase ^= 1; }
-            }
-            if (TWO) tcgen05_commit_2sm(&tmem_full_bar[as]);
-            else tcgen05_commit(&tmem_full_bar[as]);
           }
         }
       }
     }
   } else {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    // ================= epilogue = the cell (warps 4..11) =================
-    // two warps per TMEM lane quarter; warp group s owns hidden units [32 s, 32 s + 32)
-    // of the tile, i.e. G gates x 32 accumulator columns per thread
-    uint32_t it = 0;
-    const int q = warp & 3;
-    const int s = (warp - 4) >> 2;
-    const uint32_t stg = smem_u32(smem + (size_t)p.stages * stage_bytes) + (uint32_t)((warp - 4) * kCellStageBytesPerWarp);
+    // ================= consumers: wgmma, then the cell (warps 4..11) =================
+    const int s = (warp - 4) >> 2;                 // hidden units [32 s, 32 s + 32) of the tile
+    const int r_lo = 16 * (warp & 3) + (lane >> 2);  // tile rows r_lo and r_lo + 8 of this thread
+    const int u_lane = 32 * s + 2 * (lane & 3);    // + 8 j (+ 1): the thread's units in the tile
+    int stage = 0;
+    uint32_t phase = 0;
     for (long long t = 0; t < p.T; ++t) {
       const int set = (int)(t & 1);
       float* out_row[S];
@@ -266,138 +147,109 @@ __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const
       float* hp_hi = p.hplane[set ^ 1][0];
       float* hp_lo = p.hplane[set ^ 1][1];
       const float* xt = p.x + t * p.x_ts;
-      for (long long tile = group_id; tile < num_tiles; tile += n_groups) {
-        const long long m0 = (tile / tiles_n) * TILE_M + (long long)rank * BLOCK_M;
+      for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const long long m0 = (tile / tiles_n) * CELL_BLOCK_M;
         const long long u0 = (tile % tiles_n) * CELL_UNITS;
-        const long long row = m0 + q * 32 + lane;
-        // The accumulator registers start out as this row's x_t gate pre-activations: the
-        // loads are in flight while the tensor core produces the first K segment, and the
-        // Gemm's "+ 1 * x_t" (blas.py:984-1017) costs no registers or latency later.
-        float acc[G][32];
-        const long long uc = u0 + s * 32;
-        const long long so = row * p.H + uc;
-        const long long row0 = row - lane;  // first row of this warp's 32
-        if (row0 < p.B) {
-          const float* xr0 = xt + row0 * p.x_rs + uc + 4 * (lane & 7);
+        // The running sum starts out as this thread's x_t gate pre-activations (the Gemm's
+        // "+ 1 * x_t", blas.py:984-1017): the loads are in flight while the tensor core
+        // produces the first K segment.  f[g][4 j + 2 h + e] = (row r_lo + 8 h, unit u_lane + 8 j + e)
+        float f[G][16];
 #pragma unroll
-          for (int g = 0; g < G; ++g) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const long long r = 4 * i + (lane >> 3);
-              const float4 xv = (row0 + r < p.B) ? __ldcs(reinterpret_cast<const float4*>(xr0 + r * p.x_rs + g * p.H))
-                                                 : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-              acc[g][4 * i] = xv.x; acc[g][4 * i + 1] = xv.y; acc[g][4 * i + 2] = xv.z; acc[g][4 * i + 3] = xv.w;
-            }
-          }
-          if (row < p.B) {
-            // the previous states of this row/unit range are needed after the last segment
-#pragma unroll
-            for (int k = 0; k < S; ++k) asm volatile("prefetch.global.L2 [%0];" ::"l"(prev_row[k] + so));
-            // x_t of this CTA's next tile: in L2 by the time its coalesced loads are issued
-            const long long nt = tile + n_groups;
-            if (nt < num_tiles) {
-              const float* xn = xt + ((nt / tiles_n) * TILE_M + (long long)rank * BLOCK_M + q * 32 + lane) * p.x_rs +
-                                (nt % tiles_n) * CELL_UNITS + s * 32;
-              if ((nt / tiles_n) * TILE_M + (long long)rank * BLOCK_M + q * 32 + lane < p.B) {
-#pragma unroll
-                for (int g = 0; g < G; ++g) asm volatile("prefetch.global.L2 [%0];" ::"l"(xn + g * p.H));
-              }
-            }
-          }
-          // into the accumulator layout: the registers start out as this row's x_t gate
-          // pre-activations (the Gemm's "+ 1 * x_t", blas.py:984-1017)
-#pragma unroll
-          for (int g = 0; g < G; ++g) cell_to_rows(acc[g], stg, lane);
-        } else {
+        for (int h = 0; h < 2; ++h) {
+          const long long row = m0 + r_lo + 8 * h;
 #pragma unroll
           for (int g = 0; g < G; ++g)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) acc[g][j] = 0.0f;
+            for (int j = 0; j < 4; ++j) {
+              const float2 xv = row < p.B ? __ldcs(reinterpret_cast<const float2*>(xt + row * p.x_rs + g * p.H + u0 + u_lane + 8 * j))
+                                          : make_float2(0.0f, 0.0f);
+              f[g][4 * j + 2 * h] = xv.x;
+              f[g][4 * j + 2 * h + 1] = xv.y;
+            }
         }
-        for (int kb0 = 0; kb0 < num_k_blocks; kb0 += CELL_SEG_KB, ++it) {
-          const uint32_t as = it & 1u, aphase = (it >> 1) & 1u;
-          mbar_wait(&tmem_full_bar[as], aphase);
-          tcgen05_fence_after();
-          const uint32_t t_acc = tmem_base + as * CELL_TILE_N + ((uint32_t)(q * 32) << 16) + s * 32;
+        for (int kb0 = 0; kb0 < num_k_blocks; kb0 += CELL_SEG_KB) {
+          const int kb1 = min(kb0 + CELL_SEG_KB, num_k_blocks);
+          float d[G][16];
+          int prev = -1;
+          for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sbase = smem_u32(smem + (size_t)stage * stage_bytes);
+            const uint32_t a_hi = sbase, a_lo = sbase + p.a_tile_bytes;
+            // this warpgroup's 32 rows of gate g in the B tile: 32 x 128 B at g * 64 + 32 s
+            const uint32_t b_hi = sbase + 2 * p.a_tile_bytes + (uint32_t)(s * 32 * SW_BYTES);
+            const uint32_t b_lo = b_hi + p.b_tile_bytes;
+            wgmma_fence();
 #pragma unroll
-          for (int g = 0; g < G; ++g) cell_fold32(acc[g], t_acc + g * CELL_UNITS);
-          tcgen05_fence_before();
-          if (TWO) {
-            asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(
-                             smem_u32(&tmem_empty_bar[as]) & kPeerBitMask)
-                         : "memory");
-          } else {
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&tmem_empty_bar[as]))
-                         : "memory");
+            for (int k = 0; k < SW_BYTES / 32; ++k) {
+              const uint32_t ko = k * 32;
+              const uint32_t acc = (kb > kb0 || k > 0) ? 1u : 0u;
+#pragma unroll
+              for (int g = 0; g < G; ++g) {
+                const uint32_t bo = (uint32_t)(g * CELL_UNITS * SW_BYTES) + ko;
+                wgmma_m64n32k8_tf32(d[g], make_smem_desc(a_lo + ko, 16), make_smem_desc(b_hi + bo, 16), acc);
+                wgmma_m64n32k8_tf32(d[g], make_smem_desc(a_hi + ko, 16), make_smem_desc(b_lo + bo, 16), 1u);
+                wgmma_m64n32k8_tf32(d[g], make_smem_desc(a_hi + ko, 16), make_smem_desc(b_hi + bo, 16), 1u);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous k-block's products have retired: free its stage
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
-        }
-        float extra[S > G ? S - G : 1][32];  // states beyond the gate count (their values cannot reuse acc)
-        (void)extra;
-        if (row < p.B) {
+          wgmma_wait<0>();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float pv[S][4];
+          for (int g = 0; g < G; ++g)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) f[g][i] = __fadd_rn(f[g][i], d[g][i]);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const long long row = m0 + r_lo + 8 * h;
+          if (row >= p.B) continue;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const long long so = row * p.H + u0 + u_lane + 8 * j;
+            float pv[S][2], ov[S][2];
 #pragma unroll
             for (int k = 0; k < S; ++k) {
-              const float4 q4 = *reinterpret_cast<const float4*>(prev_row[k] + so + j);
-              pv[k][0] = q4.x; pv[k][1] = q4.y; pv[k][2] = q4.z; pv[k][3] = q4.w;
+              const float2 q2 = *reinterpret_cast<const float2*>(prev_row[k] + so);
+              pv[k][0] = q2.x; pv[k][1] = q2.y;
             }
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
+            for (int e = 0; e < 2; ++e) {
               float gv[G], pe[S], oe[S];
 #pragma unroll
-              for (int g = 0; g < G; ++g) gv[g] = acc[g][j + e];
+              for (int g = 0; g < G; ++g) gv[g] = f[g][4 * j + 2 * h + e];
 #pragma unroll
               for (int k = 0; k < S; ++k) pe[k] = pv[k][e];
               AB_CELL_EVAL(gv, pe, oe);  // the Elemwise nodes of the inner graph on pre = x_t + s_hs @ U
-              // the gate values of this unit are dead: the new states take their registers
 #pragma unroll
-              for (int k = 0; k < S; ++k) {
-                if (k < G) acc[k < G ? k : 0][j + e] = oe[k];
-                else extra[k >= G ? k - G : 0][j + e] = oe[k];
-              }
+              for (int k = 0; k < S; ++k) ov[k][e] = oe[k];
             }
-          }
-        }
-        if (row0 < p.B) {
-          // state by state through the shared block: rows out as full 128-byte lines; the state
-          // that feeds the next step's Gemm also as the hi/lo TF32 planes its TMA loads read
 #pragma unroll
-          for (int k = 0; k < S; ++k) {
-            float (&val)[32] = k < G ? acc[k < G ? k : 0] : extra[k >= G ? k - G : 0];
+            for (int k = 0; k < S; ++k) {
+              *reinterpret_cast<float2*>(out_row[k] + so) = make_float2(ov[k][0], ov[k][1]);
+              if (p.hs == k) {
+                // the state that feeds the next step's Gemm, also as its hi/lo TF32 planes
+                float hh[2], hl[2];
 #pragma unroll
-            for (int g = 0; g < 8; ++g)
-              sts128(stg + cell_st_off(lane, g), val[4 * g], val[4 * g + 1], val[4 * g + 2], val[4 * g + 3]);
-            __syncwarp();
-            const bool feeds = p.hs == k;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const long long r = 4 * i + (lane >> 3);
-              const float4 v = lds128(stg + cell_st_off((int)r, lane & 7));
-              if (row0 + r < p.B) {
-                const long long off = (row0 + r) * p.H + uc + 4 * (lane & 7);
-                *reinterpret_cast<float4*>(out_row[k] + off) = v;
-                if (feeds) {
-                  const float hn[4] = {v.x, v.y, v.z, v.w};
-                  float hh[4], hl[4];
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    uint32_t hb, lb;
-                    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(hn[e]));
-                    hh[e] = __uint_as_float(hb);
-                    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(hn[e] - hh[e]));
-                    hl[e] = __uint_as_float(lb);
-                  }
-                  *reinterpret_cast<float4*>(hp_hi + off) = make_float4(hh[0], hh[1], hh[2], hh[3]);
-                  *reinterpret_cast<float4*>(hp_lo + off) = make_float4(hl[0], hl[1], hl[2], hl[3]);
+                for (int e = 0; e < 2; ++e) {
+                  uint32_t hb, lb;
+                  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(ov[k][e]));
+                  hh[e] = __uint_as_float(hb);
+                  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(ov[k][e] - hh[e]));
+                  hl[e] = __uint_as_float(lb);
                 }
+                *reinterpret_cast<float2*>(hp_hi + so) = make_float2(hh[0], hh[1]);
+                *reinterpret_cast<float2*>(hp_lo + so) = make_float2(hl[0], hl[1]);
               }
             }
-            __syncwarp();
           }
         }
         // the new states of this tile are written: count the tile on its row block so that the
-        // producers of step t+1 may load those rows (all 256 epilogue threads' stores first)
+        // producer of step t+1 may load those rows (all 256 consumer threads' stores first)
         asm volatile("bar.sync 1, %0;" ::"r"(kCellEpiThreads) : "memory");
         if (warp == 4 && lane == 0) {
           __threadfence();
@@ -406,33 +258,13 @@ __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (TWO) cluster_sync_all();  // nobody signals the peer's barriers / reads its smem after this
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if (TWO) {
-      asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                   "r"(tmem_cols)
-                   : "memory");
-    } else {
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                   "r"(tmem_cols)
-                   : "memory");
-    }
-  }
 }
 
 #ifdef AB_CELL_JIT
-// NVRTC build: C-linkage entry points (looked up by name from ab_cell_scan)
+// NVRTC build: C-linkage entry point (looked up by name from ab_cell_scan)
 extern "C" __global__ void __launch_bounds__(kCellThreads, 1)
-ab_cell_scan_1cta(const __grid_constant__ CUtensorMap h00, const __grid_constant__ CUtensorMap h01,
-                  const __grid_constant__ CUtensorMap h10, const __grid_constant__ CUtensorMap h11,
-                  const __grid_constant__ CUtensorMap u0, const __grid_constant__ CUtensorMap u1,
-                  const __grid_constant__ CellParams p) { cell_scan_body<1>(h00, h01, h10, h11, u0, u1, p); }
-extern "C" __global__ void __launch_bounds__(kCellThreads, 1)
-ab_cell_scan_2cta(const __grid_constant__ CUtensorMap h00, const __grid_constant__ CUtensorMap h01,
-                  const __grid_constant__ CUtensorMap h10, const __grid_constant__ CUtensorMap h11,
-                  const __grid_constant__ CUtensorMap u0, const __grid_constant__ CUtensorMap u1,
-                  const __grid_constant__ CellParams p) { cell_scan_body<2>(h00, h01, h10, h11, u0, u1, p); }
+ab_cell_scan(const __grid_constant__ CUtensorMap h00, const __grid_constant__ CUtensorMap h01,
+             const __grid_constant__ CUtensorMap h10, const __grid_constant__ CUtensorMap h11,
+             const __grid_constant__ CUtensorMap u0, const __grid_constant__ CUtensorMap u1,
+             const __grid_constant__ CellParams p) { cell_scan_body(h00, h01, h10, h11, u0, u1, p); }
 #endif

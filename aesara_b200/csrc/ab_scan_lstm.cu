@@ -10,15 +10,15 @@
 // the whole T-step loop runs here without returning to the host:
 //
 //   * the grid is one CTA per SM (cooperative launch, all CTAs co-resident); every step
-//     the [B, 4H] pre-activation is produced as 128 x 256 tcgen05 tiles (3xTF32,
+//     the [B, 4H] pre-activation is produced as 64 x 256 wgmma tiles (3xTF32,
 //     fp32-faithful like ab_gemm) whose 256 columns are the four gates of 64 hidden units
 //     (U is packed once with its columns gate-interleaved);
-//   * the LSTM cell is the tile's epilogue: accumulators come out of TMEM, x_t and
+//   * the LSTM cell is the tile's epilogue, in the accumulator registers: x_t and
 //     c_{t-1} are read once, c_t / h_t are written to the Scan's circular output buffers
 //     and h_t is ALSO written as the hi/lo TF32 planes the next step's TMA loads — the
 //     pre-activations never touch HBM and there is no per-step pack or copy kernel;
-//     K is accumulated in 128-element segments (fresh TMEM accumulator each, summed in
-//     FP32 registers) because the tensor core's own accumulate truncates;
+//     K is accumulated in 256-element segments (fresh register accumulator each, summed
+//     in FP32) because the tensor core's own accumulate truncates;
 //   * there is no barrier between steps.  Batch rows are independent, so a tile of step
 //     t+1 only needs the h_t rows of ITS row block: every finished tile is counted on its
 //     row block (release: bar.sync of the epilogue warps, __threadfence, atomicAdd) and the
@@ -28,7 +28,7 @@
 //     the same row block read, and those are complete by then.
 //
 // State lives in L2 (h planes 2 x 2 x B x H x 4 B, c in the output ring): 8192 x 1024
-// state rows do not fit the register file / shared memory of 148 SMs at M = 128 tiles.
+// state rows do not fit the register file / shared memory of the SMs.
 #include <cooperative_groups.h>
 
 #include <algorithm>
@@ -36,7 +36,7 @@
 #include <vector>
 
 #include "ab_common.h"
-#include "ab_tcgen05.cuh"
+#include "ab_tc.cuh"
 
 namespace ab {
 
@@ -45,23 +45,23 @@ namespace {
 using namespace ab::tc;
 
 // ---- the ahead-of-time member of the family: the LSTM cell of BASELINE config 4 ----------
-// gates (i, f, o, g) = pre[:, 0:H], [H:2H], [2H:3H], [3H:4H]; states (h, c)
+// gates (i, f, o, g) = pre[:, 0:H], [H:2H], [2H:3H], [3H:4H]; states (h, c).  Products are
+// rounded on their own (no FMA contraction), as in the generated cells (codegen/scan_cell.py).
 #define AB_CELL_GATES 4
 #define AB_CELL_STATES 2
-#define AB_CELL_EVAL(G, P, O)                                                              \
-  {                                                                                        \
-    (O)[1] = sigmoidf_ref((G)[1]) * (P)[1] + sigmoidf_ref((G)[0]) * tanhf((G)[3]);          \
-    (O)[0] = sigmoidf_ref((G)[2]) * tanhf((O)[1]);                                          \
+#define AB_CELL_EVAL(G, P, O)                                                                           \
+  {                                                                                                     \
+    (O)[1] = __fmul_rn(sigmoidf_ref((G)[1]), (P)[1]) + __fmul_rn(sigmoidf_ref((G)[0]), tanhf((G)[3])); \
+    (O)[0] = __fmul_rn(sigmoidf_ref((G)[2]), tanhf((O)[1]));                                           \
   }
 #include "ab_scan_cell_kernel.cuh"
 
-template <int CTAS>
 __global__ void __launch_bounds__(kCellThreads, 1)
 lstm_scan_kernel(const __grid_constant__ CUtensorMap map_h00, const __grid_constant__ CUtensorMap map_h01,
                  const __grid_constant__ CUtensorMap map_h10, const __grid_constant__ CUtensorMap map_h11,
                  const __grid_constant__ CUtensorMap map_u0, const __grid_constant__ CUtensorMap map_u1,
                  const __grid_constant__ CellParams p) {
-  cell_scan_body<CTAS>(map_h00, map_h01, map_h10, map_h11, map_u0, map_u1, p);
+  cell_scan_body(map_h00, map_h01, map_h10, map_h11, map_u0, map_u1, p);
 }
 
 // hi/lo TF32 planes of a [R, K] row-major-able matrix; rows optionally gate-interleaved:
@@ -116,7 +116,7 @@ int make_map_f32(CUtensorMap* map, const void* base, long long k, long long rows
 }
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-inline size_t row_flag_bytes(long long b) { return align_up((size_t)((b + BLOCK_M - 1) / BLOCK_M) * 4, 256); }
+inline size_t row_flag_bytes(long long b) { return align_up((size_t)((b + CELL_BLOCK_M - 1) / CELL_BLOCK_M) * 4, 256); }
 
 }  // namespace
 }  // namespace ab
@@ -136,9 +136,8 @@ bool cell_supported(int gates, int states, long long t, long long b, long long h
          h % CELL_UNITS == 0 && b < (1LL << 31) && h < (1LL << 29) && t * (h / CELL_UNITS) * 2 < (1LL << 31);
 }
 
-// kern1 / kern2: the 1-CTA and 2-CTA instantiations (function pointers of the ahead-of-time
-// LSTM build, or kernels of an NVRTC module for a generated cell)
-int cell_scan_launch(const void* kern1, const void* kern2, int gates, int states, int hs, int64_t T,
+// kern: the ahead-of-time LSTM kernel, or the kernel of an NVRTC module for a generated cell
+int cell_scan_launch(const void* kern, int gates, int states, int hs, int64_t T,
                      int64_t B, int64_t H, const void* x, int64_t x_ts, int64_t x_rs, const void* U,
                      int64_t u_rs, int64_t u_cs, void* const* bufs, const int64_t* lens,
                      const int64_t* pos, void* workspace, size_t workspace_bytes, cudaStream_t st) {
@@ -184,72 +183,27 @@ int cell_scan_launch(const void* kern1, const void* kern2, int gates, int states
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const bool allow_2cta = getenv("AB_LSTM_1CTA") == nullptr;
-  bool two_cta = allow_2cta && kern2 && B >= 2 * BLOCK_M && sms % 2 == 0;
   CUtensorMap mh[2][2], mu[2];
   int rc;
   for (int s = 0; s < 2; ++s)
     for (int k = 0; k < 2; ++k)
-      if ((rc = make_map_f32(&mh[s][k], p.hplane[s][k], H, B, BLOCK_M))) return rc;
+      if ((rc = make_map_f32(&mh[s][k], p.hplane[s][k], H, B, CELL_BLOCK_M))) return rc;
   void* args[] = {&mh[0][0], &mh[0][1], &mh[1][0], &mh[1][1], &mu[0], &mu[1], &p};
-  p.a_tile_bytes = BLOCK_M * SW_BYTES;
-
-  if (two_cta) {
-    // a cluster of two CTAs per 256 x tile_n tile; every cluster must be co-resident (a tile of
-    // step t+1 spins on the counters of step t): cooperative launch, grid <= the occupancy query
-    p.b_tile_bytes = (tile_n / 2) * SW_BYTES;
-    const int stage_bytes = 2 * (p.a_tile_bytes + p.b_tile_bytes);
-    p.stages = std::max(2, std::min(8, (kMaxSmemGemm - 1024 - kCellStageBytes) / stage_bytes));
-    p.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(tile_n >> 3) << 17) |
-              ((uint32_t)((2 * BLOCK_M) >> 4) << 24);
-    if ((rc = make_map_f32(&mu[0], u_hi, H, (long long)gates * H, tile_n / 2))) return rc;
-    if ((rc = make_map_f32(&mu[1], u_lo, H, (long long)gates * H, tile_n / 2))) return rc;
-    AB_CUDA(cudaFuncSetAttribute(kern2, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-    const size_t smem = (size_t)p.stages * stage_bytes + 1024 + kCellStageBytes;
-    cudaLaunchConfig_t cfg{};
-    cfg.blockDim = dim3(kCellThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeCooperative;
-    attr[1].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    cfg.gridDim = dim3((unsigned)sms);
-    int max_clusters = 0;
-    cudaError_t qe = cudaOccupancyMaxActiveClusters(&max_clusters, kern2, &cfg);
-    const long long tiles2 = ((B + 2 * BLOCK_M - 1) / (2 * BLOCK_M)) * (H / CELL_UNITS);
-    if (qe == cudaSuccess && max_clusters >= 1) {
-      const long long clusters = std::max<long long>(1, std::min<long long>(tiles2, max_clusters));
-      cfg.gridDim = dim3((unsigned)(2 * clusters));
-      cudaError_t le = cudaLaunchKernelExC(&cfg, kern2, args);
-      if (le == cudaSuccess) {
-        g_launches++;
-        return AB_OK;
-      }
-    }
-    cudaGetLastError();  // cluster + cooperative launch not available here: one CTA per tile
-  }
+  p.a_tile_bytes = CELL_BLOCK_M * SW_BYTES;
   p.b_tile_bytes = tile_n * SW_BYTES;
   const int stage_bytes = 2 * (p.a_tile_bytes + p.b_tile_bytes);
-  p.stages = std::max(2, std::min(8, (kMaxSmemGemm - 1024 - kCellStageBytes) / stage_bytes));
-  p.idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(tile_n >> 3) << 17) |
-            ((uint32_t)(BLOCK_M >> 4) << 24);
+  p.stages = std::max(2, std::min(8, (kMaxSmemGemm - 1024) / stage_bytes));
   if ((rc = make_map_f32(&mu[0], u_hi, H, (long long)gates * H, tile_n))) return rc;
   if ((rc = make_map_f32(&mu[1], u_lo, H, (long long)gates * H, tile_n))) return rc;
-  AB_CUDA(cudaFuncSetAttribute(kern1, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-  const size_t smem = (size_t)p.stages * stage_bytes + 1024 + kCellStageBytes;
+  AB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
+  const size_t smem = (size_t)p.stages * stage_bytes + 1024;
   int per_sm = 0;
-  AB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern1, kCellThreads, smem));
+  AB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kCellThreads, smem));
   if (per_sm < 1) return fail(AB_ERR_CUDA, "the Scan cell kernel does not fit on an SM");
-  const long long num_tiles = ((B + BLOCK_M - 1) / BLOCK_M) * (H / CELL_UNITS);
+  const long long num_tiles = ((B + CELL_BLOCK_M - 1) / CELL_BLOCK_M) * (H / CELL_UNITS);
   // every CTA must be resident (tiles spin on the previous step's counters): cooperative, <= 1 per SM
   const unsigned grid = (unsigned)std::max<long long>(1, std::min<long long>(num_tiles, sms));
-  AB_CUDA(cudaLaunchCooperativeKernel(kern1, dim3(grid), dim3(kCellThreads), args, smem, st));
+  AB_CUDA(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(kCellThreads), args, smem, st));
   g_launches++;
   return AB_OK;
 }
@@ -274,7 +228,7 @@ extern "C" int ab_lstm_scan(int64_t T, int64_t B, int64_t H, const void* x, int6
                             void* workspace, size_t workspace_bytes, void* stream) {
   void* bufs[2] = {hbuf, cbuf};
   const int64_t lens[2] = {sh, sc}, pos[2] = {pos_h, pos_c};
-  return cell_scan_launch((const void*)lstm_scan_kernel<1>, (const void*)lstm_scan_kernel<2>, 4, 2, 0, T, B, H,
+  return cell_scan_launch((const void*)lstm_scan_kernel, 4, 2, 0, T, B, H,
                           x, x_ts, x_rs, U, u_rs, u_cs, bufs, lens, pos, workspace, workspace_bytes,
                           as_stream(stream));
 }
@@ -298,13 +252,12 @@ extern "C" int ab_cell_scan(ab_module* module, int gates, int states, int hs, in
                             size_t workspace_bytes, void* stream) {
   if (!module || !state_bufs || !state_lens || !state_pos) return fail(AB_ERR_INVALID, "null argument");
   Module* m = reinterpret_cast<Module*>(module);
-  cudaKernel_t k1 = nullptr, k2 = nullptr;
-  if (cudaLibraryGetKernel(&k1, m->lib, "ab_cell_scan_1cta") != cudaSuccess ||
-      cudaLibraryGetKernel(&k2, m->lib, "ab_cell_scan_2cta") != cudaSuccess) {
+  cudaKernel_t k = nullptr;
+  if (cudaLibraryGetKernel(&k, m->lib, "ab_cell_scan") != cudaSuccess) {
     cudaGetLastError();
     return fail(AB_ERR_INVALID, "the module is not a Scan cell build");
   }
-  return cell_scan_launch((const void*)k1, (const void*)k2, gates, states, hs, T, B, H, x, x_ts, x_rs, U,
+  return cell_scan_launch((const void*)k, gates, states, hs, T, B, H, x, x_ts, x_rs, U,
                           u_rs, u_cs, state_bufs, state_lens, state_pos, workspace, workspace_bytes,
                           as_stream(stream));
 }

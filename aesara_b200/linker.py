@@ -165,7 +165,7 @@ class B200VM:
 
 
 class B200Linker(LocalLinker):
-    """Link an optimised ``FunctionGraph`` to hand-written sm_100a kernels."""
+    """Link an optimised ``FunctionGraph`` to hand-written sm_90a kernels."""
 
     def __init__(self, allow_gc=True, precision="fp32", device_outputs=False, schedule=None,
                  cuda_graph=False, shard=None, shard_inputs=None, gather=False, host_chunks=0):

@@ -1,4 +1,4 @@
-"""Device-resident n-d arrays for the B200 runtime.
+"""Device-resident n-d arrays for the GPU runtime.
 
 A :class:`DeviceArray` is (owner, pointer, dtype, shape, element strides) —
 the device analogue of the NumPy arrays that live in the reference's storage
@@ -287,8 +287,8 @@ class DeviceArray:
     # -- host transfer ----------------------------------------------------------
     def to_numpy(self):
         """Device -> host.  Large arrays land in a page-locked block from torch's caching
-        host allocator (~53 GB/s on the B200 box; a fresh pageable array page-faults at
-        ~2.6 GB/s, profiles/r01_pcie_probe.json) and the returned ndarray owns that block
+        host allocator (a fresh pageable array page-faults on every page it receives) and
+        the returned ndarray owns that block
         through its base, so results are never recycled under the caller
         (``Out(borrow=False)`` semantics, compile/function/types.py:1067-1117)."""
         from .kernels import contiguous_copy

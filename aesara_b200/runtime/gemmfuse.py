@@ -1,7 +1,7 @@
 """GEMM-epilogue regions: ``Dot22``/``Gemm``/``Dot22Scalar`` followed by the ``Elemwise`` nodes
 that consume the product — and the ``Sum`` nodes that consume *those* — run as a single
-tcgen05 kernel whose epilogue evaluates the merged scalar program of the Elemwise nodes
-(``codegen/gemm_epilogue.py``, ``csrc/ab_gemm_tcgen05_kernel.cuh``).
+tensor-core kernel whose epilogue evaluates the merged scalar program of the Elemwise nodes
+(``codegen/gemm_epilogue.py``, ``csrc/ab_gemm_tc_kernel.cuh``).
 
 In BASELINE config 3 (SURVEY App. A.3) the regions are
 

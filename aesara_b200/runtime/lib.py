@@ -234,7 +234,7 @@ def load():
                 _build.build_library()
             except Exception as e:  # pragma: no cover
                 raise RuntimeError(
-                    f"libaesara_b200.so is missing and could not be built ({e}); the B200 "
+                    f"libaesara_b200.so is missing and could not be built ({e}); the GPU "
                     "backend has no CPU fallback"
                 ) from e
         lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
@@ -280,14 +280,16 @@ def _find_cache_dir(d):
         with open(probe, "w"):
             pass
         os.remove(probe)
-    except OSError:
-        d = os.path.join(os.path.expanduser("~"), ".cache", "aesara_b200", "kernels")
+    except OSError:  # a read-only tree: the cubins go to a temporary directory
+        import tempfile
+
+        d = os.path.join(tempfile.gettempdir(), f"aesara_b200_kernels_{os.getuid()}")
         os.makedirs(d, exist_ok=True)
     return d
 
 
 def compile_cubin(src: str, name: str = "ab_module") -> bytes:
-    """NVRTC-compile ``src`` for sm_100a (disk-cached).  Needs no GPU."""
+    """NVRTC-compile ``src`` for sm_90a (disk-cached).  Needs no GPU."""
     lib = load()
     key = hashlib.sha256((lib.ab_version().decode() + src).encode()).hexdigest()[:40]
     path = os.path.join(cache_dir(), f"{name}_{key}.cubin")

@@ -201,12 +201,10 @@ class ProgramExecutor:
 
         self._fusions = RowFusion.detect(program, self._destroys)
         taken = {i for f in self._fusions for i in f.members}
-        # GEMM-epilogue regions under the reduced-precision product policies only.  The
-        # fp32-faithful kernels (hi/lo operands, K segments folded into 128 accumulator
-        # registers per thread) have no registers left for a region's epilogue: measured on
-        # cfg3, 58.8 ms with regions against 49.3 ms node by node (the Elemwise / CAReduce
-        # kernels of the unfused graph run at the HBM roof and cost 2.5 ms of that;
-        # profiles/r02_bench_fp32_regions.json).  AB_GEMM_FUSE_FP32=1 keeps them (tests).
+        # GEMM-epilogue regions under the reduced-precision product policies only: the
+        # fp32-faithful kernels spend three tensor-core passes per product, and the Elemwise /
+        # CAReduce kernels of the unfused graph run at the HBM roof, so a region saves little
+        # there.  AB_GEMM_FUSE_FP32=1 keeps them (tests).
         if self.precision == 0 and not os.environ.get("AB_GEMM_FUSE_FP32"):
             gemm_regions = []
         else:

@@ -106,7 +106,7 @@ class B200SharedVariable(TensorSharedVariable):
 
 
 def shared(value, name=None, strict=False, allow_downcast=None, borrow=False, shape=None):
-    """``aesara.shared`` for values that should live on the B200 between calls
+    """``aesara.shared`` for values that should live on the GPU between calls
     (same arguments as ``tensor_constructor``, ``tensor/sharedvar.py:48-85``)."""
     if is_device_value(value):
         dev = value
@@ -146,7 +146,7 @@ def register_shared_constructor(ndarrays=False):
     ``tensor/sharedvar.py:48`` registers ``np.ndarray``).
 
     ``ndarrays=True``: NumPy arrays given to ``aesara.shared`` also become
-    ``B200SharedVariable``s, so an unchanged user script keeps its parameters on the B200
+    ``B200SharedVariable``s, so an unchanged user script keeps its parameters on the GPU
     between calls (their values move to the device at the first ``updates=`` of a B200
     function).  Opt-in, because a function compiled with another linker that shares such a
     variable needs ``sync_to_host()`` first.  ``ndarrays=False`` restores the default."""

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Benchmark of the hot path (BASELINE.json metric): graph-evals/s of an optimised
-Aesara graph executed by the B200 backend, measured THROUGH THE DROP-IN BOUNDARY
+Aesara graph executed by the H100 (sm_90a) backend, measured THROUGH THE DROP-IN BOUNDARY
 (``aesara.function(..., mode=B200)`` -> ``Function.__call__`` -> ``B200VM`` -> C ABI -> CUDA),
 with the roofline of its dominant kernels and the reference's own C-linker timed beside it.
 
@@ -15,8 +15,13 @@ evaluation replayed as one CUDA graph.  ``device_ms`` / ``roofline``: a second t
 of the same K steps launched eagerly with CUDA events around every node.  ``e2e``: the call a
 user makes -- page-locked host ndarrays in, host ndarrays out, copies inside the timed region.
 The front-end the plugin sits behind (graph builder + rewriter) is whichever ``aesara`` is
-importable; on the GPU box that is the travelling copy of the reference (``oracle/_ref``),
-used as the host of the plugin and as the CPU arm, never as a compute fallback.
+importable; without an installed one that is the copy of the reference ``build()`` leaves under
+``oracle/_ref``, used as the host of the plugin and as the CPU arm, never as a compute fallback.
+
+``--dump-outputs DIR`` writes what the timed path returned in its last step, one
+``DIR/<name>.npy`` per output (float32 / float64; an output too large for the 64 MB budget as a
+fixed, seeded sample of its elements), so that two builds can be compared output for output:
+the inputs are seeded and identical from run to run.
 """
 
 import argparse
@@ -275,26 +280,6 @@ class ClockSampler:
                 "samples": len(sm)}
 
 
-def ncu_traffic(summary, kernel_substr):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the kernel from
-    a committed ``ncu --set full`` summary under profiles/ (None if it is not there)."""
-    path = os.path.join(ROOT, "profiles", summary)
-    if not os.path.exists(path):
-        return None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    total, inside, seen = 0.0, False, 0
-    for line in open(path):
-        if line.startswith("kernel:"):
-            if inside and seen == 2:
-                break
-            inside, total, seen = kernel_substr in line, 0.0, 0
-        elif inside and ("dram__bytes_read.sum " in line or "dram__bytes_write.sum " in line):
-            parts = line.split()
-            total += float(parts[1]) * unit.get(parts[2], 1.0)
-            seen += 1
-    return total if seen == 2 else None
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -302,7 +287,8 @@ def measured_peaks():
             d = json.load(f)
         return dict(hbm=d["hbm_gbs"], bf16=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     bf16_burst=d["bf16_tflops"], src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, bf16=1400.0, bf16_burst=1590.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not measured
+    return dict(hbm=3350.0, bf16=989.0, bf16_burst=989.0, src="H100 SXM data sheet (not measured)")
 
 
 # ----------------------------------------------------------------------------- CPU arm
@@ -495,9 +481,32 @@ def truth_check(spec, precision, outs, keep):
             "err": err, "max_err": max(err.values()), "stated_tolerance": tol, "within": max(err.values()) <= tol}
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_outputs(outs, out_dir):
+    """Write the outputs of one evaluation as ``out_dir/out_<k>.npy`` (float32, or float64 for
+    float64 outputs).  Within the 64 MB budget an output is stored whole; a larger one as the
+    elements at a fixed, seeded, sorted set of flat indices (stored beside it as
+    ``out_<k>.index.npy``), the same set in every run of the same workload."""
+    os.makedirs(out_dir, exist_ok=True)
+    outs = list(outs) if isinstance(outs, (list, tuple)) else [outs]
+    per_out = DUMP_BUDGET_BYTES // max(1, len(outs))
+    for k, o in enumerate(outs):
+        a = o.to_numpy() if hasattr(o, "to_numpy") else np.asarray(o)
+        a = np.asarray(a, dtype=np.float64 if a.dtype == np.float64 else np.float32)
+        if a.nbytes > per_out:
+            n = per_out // (a.itemsize + 8)  # the index array shares the budget
+            idx = np.sort(np.random.default_rng(k).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(out_dir, f"out_{k}.index.npy"), idx)
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"out_{k}.npy"), a)
+
+
 def measure(spec, precision, steps, warmup, rank=0, world=1, dist=None, use_graph=True,
-            node_region=True, e2e_steps=0, seed=1234, check_truth=False):
-    """One workload on this rank's GPU.  Returns a dict of measurements (see main())."""
+            node_region=True, e2e_steps=0, seed=1234, check_truth=False, dump_dir=None):
+    """One workload on this rank's GPU.  Returns a dict of measurements (see main()).
+    ``dump_dir``: where the outputs of the last timed step go (dump_outputs)."""
     import torch
 
     from aesara_b200.runtime import lib
@@ -519,14 +528,17 @@ def measure(spec, precision, steps, warmup, rank=0, world=1, dist=None, use_grap
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = []
+
     def timed_region(n):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
         e0.record()
         for _ in range(n):
-            step()
+            out = step()
         e1.record()
         barrier()
+        last[:] = [out]
         t = torch.tensor([e0.elapsed_time(e1)], device="cuda")
         if dist is not None:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -547,6 +559,8 @@ def measure(spec, precision, steps, warmup, rank=0, world=1, dist=None, use_grap
     l0 = L.ab_launch_count()
     ms_step = timed_region(steps)
     launches = L.ab_launch_count() - l0
+    if dump_dir is not None:
+        dump_outputs(last[0], dump_dir)
     replay = getattr(getattr(f, "vm", None), "_replay", None) or getattr(f, "replay", None)
     replayed = bool(replay is not None and replay.replays)
     res.update(ms_per_step=ms_step, executor="cuda-graph replay" if replayed else "eager launches")
@@ -739,8 +753,8 @@ def roofline_of(spec, precision, m, peaks):
         ach = spec["gemm_flops"] / (t * 1e-3) / 1e12
         peak = peaks["bf16"] if precision == "bf16" else peaks["bf16"] / 2.0
         r = {"bound": "tensor",
-             "kernel": ("ab_lstm_scan (persistent 2-CTA tcgen05 Scan kernel)" if spec["name"] == "lstm" else
-                        "tcgen05 GEMM launches (+operand packs) of the Gemm/Dot22 nodes, consumer Elemwise fused in"),
+             "kernel": ("ab_lstm_scan (persistent wgmma Scan kernel)" if spec["name"] == "lstm" else
+                        "wgmma GEMM launches (+operand packs) of the Gemm/Dot22 nodes, consumer Elemwise fused in"),
              "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
              "peak_source": peaks["src"] + (" sustained bf16" if precision == "bf16"
                                             else "; tf32 = bf16/2 (nominal ratio)"),
@@ -789,6 +803,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="skip the one-liners of the other configs")
     ap.add_argument("--no-truth", action="store_true", help="skip the float64 parity check of the headline run")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/out_<k>.npy (rank 0)")
     args = ap.parse_args()
     spec = workload_spec(args.workload, args.batch, args.hidden, args.n, args.steps_t)
     if args.precision is None:
@@ -819,22 +835,10 @@ def main():
             raise SystemExit(f"sharded evaluation disagrees with the single-GPU one: {parity}")
     m = measure(spec, args.precision, args.steps, args.warmup, rank, world, dist,
                 use_graph=bool(args.graph), e2e_steps=0 if args.no_e2e else max(2, min(args.steps, 5)),
-                check_truth=not args.no_truth)
+                check_truth=not args.no_truth, dump_dir=args.dump_outputs if rank == 0 else None)
     ms_step = m["ms_per_step"]
     value = world * 1e3 / ms_step  # every rank evaluates its shard once per step
     roofline = roofline_of(spec, args.precision, m, peaks)
-
-    # DRAM traffic of the dominant kernel, per launch, from the committed ncu --set full summary
-    tsrc = None
-    if spec["name"] == "mlp" and args.precision == "bf16":
-        tsrc = ("r02_bench_step_ncu_v4.txt", "ab_gemm_ep_2cta_f16")  # first launch of the capture: region 3
-    elif spec["name"] == "logreg" and m["fused_regions_run"] > 0:
-        tsrc = ("r01_rowfused_logreg.txt", "ab_rowfused")
-    elif spec["name"] == "elemwise":
-        tsrc = ("r01_elemwise_cfg2_v2_unroll1.txt", "ab_ew_flat_vec")
-    if tsrc is not None:
-        roofline["traffic"] = ncu_traffic(*tsrc)
-        roofline["traffic_source"] = f"profiles/{tsrc[0]} ({tsrc[1]}, dram__bytes_read.sum + dram__bytes_write.sum per launch)"
 
     also = None
     if rank == 0 and world == 1 and not args.no_also and args.workload == "mlp":
@@ -876,7 +880,7 @@ def main():
             "data": "synthetic",
             "config": {"workload": spec["desc"], "parallelism": par, "boundary": m["boundary"],
                        "l2": ("working set fits L2: launch-latency bound, reported as evals/s only"
-                              if spec["name"] == "readme" else "inputs >> 126 MB L2, no flush needed"),
+                              if spec["name"] == "readme" else "inputs >> 50 MB L2, no flush needed"),
                        "executor": m["executor"],
                        "gemm_precision": args.precision if spec["n_gemm"] else None,
                        "stated_tolerance": (f"norm-wise rtol {TOLERANCE[args.precision]} vs the reference "

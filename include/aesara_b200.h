@@ -1,4 +1,4 @@
-/* aesara_b200.h — C ABI of libaesara_b200.so, the B200 (sm_100a) device runtime
+/* aesara_b200.h — C ABI of libaesara_b200.so, the H100 (sm_90a) device runtime
  * behind Aesara's Linker/Op plugin surface.
  *
  * Conventions (they mirror the reference's native thunk ABI,
@@ -83,7 +83,7 @@ int ab_event_elapsed_ms(void* start, void* stop, float* ms);
 int ab_event_destroy(void* ev);
 
 /* ---- JIT: generated kernel per fused Elemwise{Composite} / CAReduce ------ */
-/* Compile CUDA C++ to an sm_100a cubin with NVRTC.  Needs no GPU.  Replaces
+/* Compile CUDA C++ to an sm_90a cubin with NVRTC.  Needs no GPU.  Replaces
  * GCC_compiler.compile_str (aesara/link/c/cmodule.py:2482).  *cubin is
  * malloc()ed; release with ab_buffer_free. */
 int ab_nvrtc_compile(const char* src, const char* name, const char* const* extra_opts,
@@ -128,7 +128,7 @@ int ab_careduce_launch(ab_module* m, int ndim, const int64_t* shape, const int64
  * Gemm / Dot22 (aesara/tensor/blas.py:872 / :1659, C template :518-869):
  *   C[m,n] <- beta*C + alpha * A[m,k] @ B[k,n]; arbitrary 2-D element strides
  *   (the eight stride cases of blas.py:765-776 plus copies for the rest);
- *   tcgen05/TMEM tensor-core tiles fed by TMA.  `precision`:
+ *   wgmma tensor-core tiles fed by TMA.  `precision`:
  *     0 = fp32-faithful (3xTF32 split, rtol 1e-5 vs sgemm),
  *     1 = single TF32 pass, 2 = BF16 operands / FP32 accumulate (policy mode).
  *   dtype is AB_F32 or AB_F64 (the only dtypes the reference Gemm accepts,
@@ -154,7 +154,7 @@ int ab_gemm_workspace_bytes(int dtype, int precision, int64_t m, int64_t n, int6
  * it once: logical operand [rows, k] (rows = M for A, N for B; element strides
  * s_r, s_k) -> ab_gemm_operand, then ab_gemm_packed.  A transposed view of the
  * same memory yields the same planes with mn_major flipped, so one pack serves
- * both products (the operand is handed to tcgen05.mma as MN-major). */
+ * both products (the operand is handed to wgmma as MN-major). */
 typedef struct {
   const void* plane0;   /* hi / only plane */
   const void* plane1;   /* lo plane of the 3xTF32 split, else NULL */
@@ -186,7 +186,7 @@ int ab_gemm_packed(int precision, int64_t m, int64_t n, int64_t k, double alpha,
 int ab_gemm_packed_workspace_bytes(int precision, int64_t m, int64_t n, int64_t k, size_t* bytes);
 
 /* Gemm/Dot22 followed by the Elemwise (and Sum) nodes that consume it, in one kernel:
- * `module` is the NVRTC build of the tcgen05 kernels with the scalar program of those nodes
+ * `module` is the NVRTC build of the tensor-core GEMM kernels with the scalar program of those nodes
  * as the epilogue (aesara_b200/codegen/gemm_epilogue.py).  Per element the program maps
  * v = beta*Cin + alpha*A@B and the operands e_i = ptr[i][row*rs[i] + col*cs[i]] (stride 0
  * broadcasts) to n_outputs values.  Value 0 is stored to C (C may be NULL: not stored),
@@ -271,7 +271,7 @@ int ab_cumulative(int dtype, int mul, const void* x, void* out, int64_t outer, i
 /* ---- Scan fast path: LSTM-cell recurrence as one persistent kernel -----------------
  * (aesara/scan/op.py:637; inner graph of SURVEY App. A.4).  For t in [0,T):
  *   pre = x[t] + h_{t-1} @ U;  c_t = sigmoid(pre_f)*c_{t-1} + sigmoid(pre_i)*tanh(pre_g);
- *   h_t = sigmoid(pre_o)*tanh(c_t)      (gate column order i, f, o, g; 3xTF32 tcgen05 tiles)
+ *   h_t = sigmoid(pre_o)*tanh(c_t)      (gate column order i, f, o, g; 3xTF32 wgmma tiles)
  * hbuf / cbuf are the Scan's circular output buffers [sh|sc, B, H] (contiguous); the row
  * before pos_h / pos_c holds the initial state; step t writes row (pos + t) % s.
  * x is [T, B, 4H] with element strides (x_ts, x_rs, 1); U is [H, 4H] with strides

@@ -8,7 +8,7 @@ for sigmoid / softplus / log1mexp).  Evaluates the IR scalar expressions of
 
 Pinned against the reference itself: ``tests/golden/make_golden.py`` runs the real
 reference (C-linker ``Mode("cvm")``; its Python ``perform`` for the few Ops whose C code no
-longer builds on NumPy 2) in the build container on seeded inputs and commits programs,
+longer builds on NumPy 2) on seeded inputs and commits programs,
 inputs and reference outputs under ``tests/golden/``; ``tests/test_oracle.py`` checks this
 oracle against every one of them.
 """

@@ -7,15 +7,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-# the reference front-end the linker plugs into: the travelling copy under oracle/_ref (made by
-# __graft_entry__.build() in the build container), never /root/reference on the GPU box
+# the reference front-end the linker plugs into: the copy under oracle/_ref that
+# __graft_entry__.build() makes (oracle/ref.py)
 from oracle import ref as _ref  # noqa: E402
 
 _ref.activate()
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "reference: needs the reference front-end (oracle/_ref)")
 
 

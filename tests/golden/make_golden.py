@@ -1,7 +1,7 @@
 """Generate the golden fixtures under tests/golden/ with the REFERENCE itself.
 
-Run in the build container only (it imports /root/reference through the
-overlay in aesara_b200.compat):
+Run where a checkout of the reference is available (it imports it through the
+overlay in aesara_b200.compat, see oracle/ref.py):
 
     PYTHONPATH=. python tests/golden/make_golden.py
 

@@ -1,6 +1,6 @@
 """CPU, world_size 2 over gloo: the host-side sharding logic (row blocks, packed
 exchange layout, mean-of-shards weights) reproduces the unsharded result.  The
-per-shard evaluation uses the oracle interpreter here; on the GPU box the same
+per-shard evaluation uses the oracle interpreter here; on the GPU the same
 logic drives the device executor (bench.py --gpus N)."""
 import os
 import socket

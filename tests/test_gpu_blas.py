@@ -64,11 +64,12 @@ def test_gemm_fp32_faithful(K, m, n, k, layout):
 @pytest.mark.parametrize("layout", ["nn", "tn", "nt", "tt"])
 @pytest.mark.parametrize("m,n,k", [(1024, 256, 192), (1500, 520, 1000), (4096, 1024, 512), (2300, 256, 4160)])
 def test_gemm_four_cta_cluster_multicast(K, m, n, k, layout, precision):
-    """With AB_GEMM_CLUSTER4 set, M >= 1024 takes the 4-CTA cluster kernel (two CTA pairs sharing
-    the B tile by TMA multicast).  Its per-element arithmetic is the 2-CTA kernel's, so the result must be
-    BIT-IDENTICAL to the 2-CTA path (AB_GEMM_NO_CLUSTER4) for every operand layout (K-major and
-    MN-major B quarters), ragged cluster tiles (second pair partly or wholly out of range) and
-    both the 3xTF32 and bf16 policies; and inside tolerance of a float64 product."""
+    """With AB_GEMM_CLUSTER4 set, M >= 1024 takes the 4-CTA cluster kernel (four CTAs stacked along
+    M sharing the B tile: each loads a quarter and multicasts it to all four).  Its per-element
+    arithmetic is the single-CTA kernel's, so the result must be BIT-IDENTICAL to the default path
+    for every operand layout (K-major and MN-major B quarters), ragged cluster tiles (trailing CTAs
+    partly or wholly out of range) and both the 3xTF32 and bf16 policies; and inside tolerance of a
+    float64 product."""
     import os
 
     rng = np.random.default_rng(m + n + k)

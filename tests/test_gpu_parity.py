@@ -283,7 +283,7 @@ def _fused_vs_plain(fused, plain, what, exact_sums=True):
 @pytest.mark.parametrize("precision", [0, 2])
 def test_mlp_gemm_epilogue_fusion_matches_node_by_node(rt, precision, monkeypatch):
     """cfg3 graph, B=1024, H=512: the three Gemm/Dot22 -> Elemwise pairs run as fused
-    tcgen05 kernels (runtime/gemmfuse.py) and give the node-by-node result (the epilogue
+    tensor-core kernels (runtime/gemmfuse.py) and give the node-by-node result (the epilogue
     evaluates the same scalar expression on the same fp32 values; the bf16 shadow plane it
     writes equals the separate pack, so even the bf16 policy is bit-identical)."""
     import os
@@ -332,7 +332,7 @@ def test_mlp_gemm_epilogue_fusion_matches_node_by_node(rt, precision, monkeypatc
 def test_mlp_gemm_epilogue_fusion_ragged_batch(rt, precision, B, monkeypatch):
     """cfg3 graph with a batch that is not a multiple of the 32-row chunks / 128-row tiles of the
     fused epilogue (last warp partly outside, last tile partly outside, odd K of the weight
-    gradients; B=4099 takes the 2-CTA kernel): staged row stores, column sums over partly
+    gradients; B=4099 spans 33 row tiles): staged row stores, column sums over partly
     empty 32-row blocks and the transposed bf16 plane's ragged rows give the node-by-node
     result."""
     import os
@@ -358,8 +358,8 @@ def test_mlp_gemm_epilogue_fusion_ragged_batch(rt, precision, B, monkeypatch):
 
 @pytest.mark.parametrize("T,B,H", [(12, 256, 128), (5, 384, 192), (4, 200, 64)])
 def test_lstm_medium_size_vs_oracle_and_graph_replay(rt, T, B, H):
-    """cfg4 graph at medium sizes (a full 2-CTA tile, a ragged second 2-CTA tile, and a
-    batch below 256 that takes the 1-CTA kernel): eager device loop == oracle; the
+    """cfg4 graph at medium sizes (full 64-row tiles, a ragged last tile, and a batch that
+    is not a multiple of 8): eager device loop == oracle; the
     CUDA-graph replay of the whole evaluation returns bit-identical results."""
     from oracle.program_np import run_program
     from aesara_b200.runtime.device import DeviceArray
@@ -525,7 +525,7 @@ def test_lstm_full_size_fast_path_vs_general_loop(rt):
 def test_gemm_full_size_tile_independence(rt):
     """BASELINE-size GEMM property (no CPU truth at this size): rows of a
     [16384, 4096] x [4096, 4096] product equal the product of the row subset, for
-    both the 2-CTA and the ragged-tail tile paths; bf16 result is within 2e-2 of the
+    both full and ragged-tail tiles; bf16 result is within 2e-2 of the
     fp32-faithful one."""
     import torch
 
@@ -583,7 +583,7 @@ def test_scan_cell_family_runs_as_one_persistent_kernel(rt, name, gates):
     for k, (g, e) in enumerate(zip(got, general)):
         assert_matches(g, e, blas=True, what=f"{name} output {k}: persistent kernel vs general loop")
     assert fast_launches < slow_launches
-    # larger, ragged shapes against the oracle (second 2-CTA tile partly empty; 1-CTA kernel)
+    # larger, ragged shapes against the oracle (last 64-row tile partly empty)
     rng = np.random.default_rng(gates)
     for T, B, H in ((9, 384, 128), (4, 200, 64)):
         vals = [rng.standard_normal((T, B, gates * H)).astype("float32"),

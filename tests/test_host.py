@@ -43,7 +43,7 @@ def test_no_device_is_a_loud_error():
 
 
 @pytest.mark.parametrize("name", ["cfg2_fused", "cfg3_mlp", "cfg5_logreg", "ew_int_arith"])
-def test_kernels_compile_for_sm100a_without_gpu(name):
+def test_kernels_compile_for_sm90a_without_gpu(name):
     from aesara_b200.runtime.vm import ProgramExecutor
 
     prog, _, _ = load_case(name)
@@ -180,7 +180,7 @@ def test_cell_matcher_family_and_rejections():
         assert spec is not None and not spec.is_lstm and (spec.gates, spec.states, spec.hs) == (gates, states, 0)
 
 
-def test_generated_scan_cells_compile_for_sm100a():
+def test_generated_scan_cells_compile_for_sm90a():
     """NVRTC (no GPU): the persistent Scan kernel with cells generated from inner graphs."""
     for name, gates in (("scan_rnn_tanh_cell", 1), ("scan_gated_unit_cell", 3), ("cfg4_lstm", 4)):
         spec = _scan_runner(name).cell.match(256, 64, gates)
@@ -245,8 +245,8 @@ def test_fusion_regions_detected_on_the_committed_programs():
         assert not [f for f in ProgramExecutor(prog)._fusions if type(f).__name__ == "RowFusion"]
 
 
-def test_fused_kernel_sources_compile_for_sm100a():
-    """NVRTC (no GPU needed): the row-region kernel, the tcgen05 GEMM with a generated
+def test_fused_kernel_sources_compile_for_sm90a():
+    """NVRTC (no GPU needed): the row-region kernel, the wgmma GEMM with a generated
     epilogue, and the reduction with a fused pre-map."""
     from aesara_b200.runtime.vm import ProgramExecutor
     from tests._cases import load_case
@@ -308,14 +308,14 @@ def test_gemm_epilogue_sources_follow_the_precision_policy(monkeypatch):
             tf.write(cubin)
             tf.flush()
             out = subprocess.run(["cuobjdump", "-res-usage", tf.name], capture_output=True, text=True).stdout
-        m = re.search(r"Function ab_gemm_ep_2cta_f16:\s*\n\s*REG:(\d+) STACK:(\d+)", out)
+        m = re.search(r"Function ab_gemm_ep_f16:\s*\n\s*REG:(\d+) STACK:(\d+)", out)
         assert m is not None, out[:400]
         assert int(m.group(2)) <= 128, f"stack frame of the fused bf16 kernel: {m.group(0)}"  # was 184-264 with spills in the chunk loop
 
 
 def test_staging_swizzle_is_conflict_free():
-    """The shared-memory chunk of the fused GEMM epilogue / Scan cell epilogue (st_off in
-    csrc/ab_gemm_tcgen05_kernel.cuh, cell_st_off in ab_scan_cell_kernel.cuh): 32 rows x 32 floats,
+    """The shared-memory chunk of the fused GEMM epilogue (st_off in
+    csrc/ab_gemm_tc_kernel.cuh): 32 rows x 32 floats,
     16-byte group g of row r stored at group g ^ (r & 7).  Restated here: every access pattern the
     kernels use touches each of the 32 banks at most once per shared-memory wavefront (128-bit
     accesses are served a quarter warp = 8 lanes at a time, 32-bit accesses a whole warp)."""

@@ -5,7 +5,7 @@ give Function-level semantics identical to the reference VM (storage cells,
 shared-variable updates, output order).  No GPU here, so the *device executor*
 is replaced by the oracle interpreter for these tests only — what is under test
 is the linker/VM glue and the lowering, not the kernels (tests/test_gpu_parity.py
-covers those on the B200 box)."""
+covers those on the GPU)."""
 import numpy as np
 import pytest
 
@@ -106,7 +106,7 @@ def _same_program(a, b, path="program"):
 @pytest.mark.parametrize("cfg", ["cfg1_readme", "cfg2_fused", "cfg3_mlp", "cfg5_logreg", "cfg4_lstm"])
 def test_linker_path_lowers_to_the_committed_fixture(aes, cfg):
     """What ``aesara.function(..., mode="B200")`` links — outer graph AND the inner graph of
-    a Scan — is the program committed under tests/golden (which the GPU box replays), and it
+    a Scan — is the program committed under tests/golden (which the GPU tests replay), and it
     does not depend on another linker having compiled the Scan first (ADVICE r1: the inner
     graph is rewritten by lower.optimized_inner_fgraph, never by a side effect of op.fn)."""
     aesara, L = aes
