@@ -12,15 +12,17 @@
 //   precision 2  BF16 operands, FP32 accumulation (the "bf16 compute policy"
 //                of BASELINE config 3; stated looser rtol).
 //
-// Structure (one 128 x 128 output tile at a time per CTA, persistent, 384 threads):
+// Structure (one 128 x 128 output tile at a time per CTA, persistent, 512 threads):
 //   warpgroup 0   TMA producer: cp.async.bulk.tensor 2-D loads of 128-byte-swizzled
 //                 operand tiles into a multi-stage smem ring, completion on mbarriers
 //                 (expect_tx);
 //   warpgroups 1-2  wgmma.mma_async (M = 64 rows each, N = 128) from the ring into
-//                 register accumulators, every finished K segment added into the tile's
-//                 float32 accumulator in shared memory; then the epilogue reads it with one
-//                 row per lane, applies alpha/beta (or the fused region) and stores C with
-//                 arbitrary strides.
+//                 register accumulators, every finished K segment added into a running
+//                 total in registers, stored once per tile into a float32 accumulator in
+//                 shared memory;
+//   warpgroup 3   epilogue: reads that accumulator with one row per lane, applies
+//                 alpha/beta (or the fused region) and stores C with arbitrary strides,
+//                 while warpgroups 1-2 run the next tile's main loop.
 //
 // Operands that are not K-major / 16-byte-pitched in global memory (the
 // DimShuffle{1,0} views of the MLP backward pass, blas.py:719-726 "unit" cases)

@@ -1,28 +1,40 @@
 // ab_gemm_tc_kernel.cuh — device code of the Hopper tensor-core GEMM (parameters, TMA producer,
-// wgmma consumer warpgroups, epilogue).  Included by ab_gemm_tc.cu (ahead-of-time kernels with
+// wgmma warpgroups, epilogue warpgroup).  Included by ab_gemm_tc.cu (ahead-of-time kernels with
 // the plain alpha/beta epilogue) and, with AB_EPILOGUE defined, concatenated behind a generated
 // `ab_ep_body` and compiled by NVRTC (codegen/gemm_epilogue.py): the Elemwise node that consumes
 // a Gemm/Dot22 result is then applied to the accumulator before the only store.
 #pragma once
 
-// Thread layout (384 threads, one 128 x BLOCK_N output tile at a time, persistent): warpgroup 0
-// = TMA producer (one elected thread of warp 0; warps 1..3 idle), shrunk to 24 registers;
-// warpgroups 1 and 2 = consumers, grown to 240 (setmaxnreg; 128 * 24 + 256 * 240 = 64 512 <=
-// 65 536): the larger generated epilogue regions spill below that.  Consumer warpgroup c issues the wgmma of tile rows
-// [64 c, 64 c + 64) into 64 accumulator registers per thread, adds each finished K segment
-// into the tile's float32 accumulator in shared memory, and then all eight consumer warps run
-// the epilogue from there with one row per lane (warp w: rows 32 (w % 4) .., half w / 4 of the
-// columns) -- the layout the generated epilogue regions are written for.
+// Thread layout (512 threads, one 128 x BLOCK_N output tile at a time, persistent):
+//   warpgroup 0     TMA producer (one elected thread of warp 0; warps 1..3 idle);
+//   warpgroups 1-2  MMA: warpgroup c issues the wgmma of tile rows [64 c, 64 c + 64) into 64
+//                   accumulator registers per thread and adds each finished K segment into a
+//                   running total held in 64 more registers; at the end of the unit it stores
+//                   the total ONCE into the tile's float32 accumulator in shared memory;
+//   warpgroup 3     epilogue: warp q reads tile rows [32 q, 32 q + 32) of that accumulator,
+//                   one row per lane, all BLOCK_N columns (the layout the generated epilogue
+//                   regions are written for), while the MMA warpgroups run the next unit's
+//                   main loop.
+// The shared accumulator is a single hand-off buffer between the two sides (mbarriers
+// acc_full: one arrival per MMA warp after its stores; acc_empty: one arrival per epilogue
+// warp after its last read): the MMA side needs it again only at the end of its next unit.
+// Registers (setmaxnreg, multiples of 8; 512 threads launch with 128 each = 65 536):
+//   producer 24, MMA 160 (d[64] + tot[64] + addressing), epilogue 168:
+//   128 * 24 + 256 * 160 + 128 * 168 = 3 072 + 40 960 + 21 504 = 65 536.
+// The cluster variant's producer, which multicasts, keeps 56 and its (plain) epilogue 136:
+//   128 * 56 + 256 * 160 + 128 * 136 = 7 168 + 40 960 + 17 408 = 65 536.
 constexpr int kGemmThreads = kThreads;
-constexpr int kEpiWarp0 = 4;
-// (the cluster variant's producer, which multicasts, keeps 56: 128 * 56 + 256 * 224 = 64 512)
+constexpr int kMmaWarp0 = 4;   // first warp of the MMA warpgroups
+constexpr int kEpiWarp0 = 12;  // first warp of the epilogue warpgroup
 #define AB_SETMAXNREG_CONTROL(CL)                                         \
   if (CL > 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");        \
   else asm volatile("setmaxnreg.dec.sync.aligned.u32 24;")
+#define AB_SETMAXNREG_MMA(CL) asm volatile("setmaxnreg.inc.sync.aligned.u32 160;")
 #define AB_SETMAXNREG_EPILOGUE(CL)                                        \
-  if (CL > 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");       \
-  else asm volatile("setmaxnreg.inc.sync.aligned.u32 240;")
-constexpr int kEpiThreads = 256;  // 8 consumer / epilogue warps
+  if (CL > 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 136;");       \
+  else asm volatile("setmaxnreg.inc.sync.aligned.u32 168;")
+constexpr int kMmaThreads = 256;  // 8 MMA warps
+constexpr int kEpiThreads = 128;  // 4 epilogue warps
 constexpr int BLOCK_N = 128;
 constexpr int kAccBytes = BLOCK_M * BLOCK_N * 4;  // the tile's float32 accumulator in shared memory
 
@@ -124,13 +136,13 @@ __device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* map, 
 // toward zero), a bias that grows linearly with the number of accumulation steps; an
 // unsegmented 3xTF32 K = 4096 product drifts well past a true-fp32 sgemm
 // (tests/test_gpu_blas.py::test_gemm_long_k_accuracy).  So the K loop is cut into segments of
-// seg_kblocks k-blocks: each segment starts a fresh register accumulator, and the consumer
-// warpgroup adds the finished segment into the tile's float32 accumulator in shared memory
+// seg_kblocks k-blocks: each segment starts a fresh register accumulator, and the MMA
+// warpgroup adds the finished segment into the unit's float32 total (registers, acc_fold)
 // with round-to-nearest.  For precision 0 a segment is 128 K elements (48 truncating steps);
 // the tf32 / bf16 policies use segments of 16 k-blocks (512 / 1024 K elements), so that a long
 // K (a weight gradient over a 65536-row batch) does not depend on the order of its rows beyond
 // the rounding of those folds.
-constexpr int kAccRegs = BLOCK_N / 2;  // accumulator columns per epilogue thread (half a tile row)
+constexpr int kAccRegs = BLOCK_N / 2;  // accumulator columns the plain epilogue holds at once (half a tile row)
 
 // shared-memory accumulator: [BLOCK_M][BLOCK_N] float32, 16-byte group g of row r stored at
 // group (g & ~7) | ((g ^ r) & 7) -- conflict-free for the row-per-lane reads of the epilogue
@@ -138,22 +150,34 @@ __device__ __forceinline__ uint32_t acc_off(int r, int c) {
   const int g = c >> 2;
   return (uint32_t)(r * (BLOCK_N * 4) + (((g & ~7) | ((g ^ r) & 7)) << 4) + ((c & 3) << 2));
 }
-// add (or, for the first segment, store) the warpgroup's 64 x BLOCK_N register accumulator
-__device__ __forceinline__ void acc_fold(uint32_t acc_base, const float (&d)[64], int row0, int lane, bool first) {
+// add a finished segment into the warpgroup's running total, kept in registers beside the
+// wgmma accumulator.  A unit's total starts at -0.0f, the identity of the round-to-nearest
+// add (-0 + x == x for every x, zeros of either sign included): the first segment is added
+// like the others, so the fold is one FADD per register in place (a select between d and the
+// sum costs a second copy of the total and spills it)
+__device__ __forceinline__ void acc_fold(float (&tot)[64], const float (&d)[64]) {
 #pragma unroll
-  for (int j = 0; j < BLOCK_N / 8; ++j) {
+  for (int i = 0; i < 64; ++i) tot[i] = __fadd_rn(tot[i], d[i]);
+}
+// the warpgroup's 64 x BLOCK_N total of a unit -> the tile's accumulator in shared memory
+// (acc_off layout).  Element 4 j + 2 h + e of the fragment is row row0 + lane / 4 + 8 h, column
+// 8 j + 2 (lane % 4) + e, and row0 % 8 == 0: the swizzle term (g ^ r) & 7 depends only on the
+// lane and on j % 4.  So four addresses per thread and immediate offsets cover the 32 stores
+// (32 addresses from acc_off are hoisted out of the unit loop and take registers from tot).
+__device__ __forceinline__ void acc_store(uint32_t acc_base, const float (&tot)[64], int row0, int lane) {
+  const uint32_t y = (uint32_t)(((lane >> 1) & 1) ^ (lane >> 2));  // ((column / 4) ^ row) % 8 at j = 0
+  const uint32_t base = acc_base + (uint32_t)((row0 + (lane >> 2)) * (BLOCK_N * 4) + ((lane & 1) << 3));
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = row0 + (lane >> 2) + 8 * h, c = 8 * j + 2 * (lane & 3);
-      const uint32_t a = acc_base + acc_off(r, c);
-      float x = d[4 * j + 2 * h], y = d[4 * j + 2 * h + 1];
-      if (!first) {
-        float ox, oy;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ox), "=f"(oy) : "r"(a) : "memory");
-        x = __fadd_rn(ox, x);
-        y = __fadd_rn(oy, y);
-      }
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+  for (int jj = 0; jj < 4; ++jj) {
+    const uint32_t a = base + ((y ^ (uint32_t)(2 * jj)) << 4);
+#pragma unroll
+    for (int jq = 0; jq < BLOCK_N / 32; ++jq) {
+      const int j = 4 * jq + jj;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + (uint32_t)(jq * 128 + h * 8 * BLOCK_N * 4)),
+                     "f"(tot[4 * j + 2 * h]), "f"(tot[4 * j + 2 * h + 1])
+                     : "memory");
     }
   }
 }
@@ -377,23 +401,16 @@ struct EpilogueOut {
   // matrices) and the evaluation takes column j's value from lane j by shuffle.  Read through
   // ld8 per column group instead, every one of the four groups of a chunk waits for an L2
   // round trip (L1 is swept by the matrix reads).
-  // AB_EP_ROWMASK: operands known at code-generation time to be [1, N] rows.  Those are read as
-  // 32 values per lane with eight 128-bit loads at a warp-uniform address (one wavefront each, L1
-  // hits after the first warp of the CTA), a chunk ahead, instead of one value per lane plus 32
-  // SHFL.IDX per chunk at the point of use.  A row operand that is only
-  // recognised at run time keeps the one-register shuffle path.
+  // AB_EP_ROWMASK: operands known at code-generation time to be [1, N] rows.  Those are read
+  // 8 values at a time with two 128-bit loads at a warp-uniform address (one wavefront each, L1
+  // hits after the first warp of the CTA) at the point of use, instead of one value per lane plus
+  // 32 SHFL.IDX per chunk.  Not read a chunk ahead: 32 more live registers per row operand
+  // make the dout region spill within the epilogue warpgroup's 168.  A row operand that is
+  // only recognised at run time keeps the one-register shuffle path.
 #ifndef AB_EP_ROWMASK
 #define AB_EP_ROWMASK 0
 #endif
-  static __device__ __forceinline__ constexpr int popc4(unsigned m) {  // NVRTC has no __builtin_popcount
-    return (int)((m & 1u) + ((m >> 1) & 1u) + ((m >> 2) & 1u) + ((m >> 3) & 1u));
-  }
-  static constexpr int kRowOps = ((AB_EP_ROWMASK) & 1) + (((AB_EP_ROWMASK) >> 1) & 1) +
-                                 (((AB_EP_ROWMASK) >> 2) & 1) + (((AB_EP_ROWMASK) >> 3) & 1);
   static __device__ __forceinline__ constexpr bool is_row_op(int k) { return ((AB_EP_ROWMASK >> k) & 1) != 0; }
-  static __device__ __forceinline__ constexpr int row_slot(int k) {
-    return popc4((unsigned)AB_EP_ROWMASK & ((1u << k) - 1u));
-  }
   struct ChunkPre {
     // [M, N] reads of the next chunk.  Register-only builds: this lane's row, 32 columns.
     // AB_EP_STAGED builds: the COALESCED layout -- q[i] = row 4 i + lane / 8 of the warp's 32,
@@ -416,7 +433,6 @@ struct EpilogueOut {
 #endif
 #endif
     float vec[AB_EP_NOPS > 0 ? AB_EP_NOPS : 1];
-    float rowv[kRowOps > 0 ? kRowOps : 1][32];
   };
   __device__ __forceinline__ void prefetch_chunk(ChunkPre& pre, long long row, long long col0, bool live,
                                                  const FusedScalars& sc, int lane) const {
@@ -424,16 +440,7 @@ struct EpilogueOut {
     (void)r; (void)sc; (void)pre; (void)col0;
 #pragma unroll
     for (int k = 0; k < AB_EP_NOPS; ++k) {
-      if (is_row_op(k) && sc.vec[k]) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          // N % 8 == 0 and 16-byte aligned rows (the fused launch's contract)
-          const float4 q = (col0 + j < p.N) ? __ldg(reinterpret_cast<const float4*>(p.ep_ptr[k] + col0 + j))
-                                            : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-          float* d = &pre.rowv[row_slot(k)][j];
-          d[0] = q.x; d[1] = q.y; d[2] = q.z; d[3] = q.w;
-        }
-      } else if (sc.vec[k]) {
+      if (sc.vec[k] && !is_row_op(k)) {
         pre.vec[k] = (col0 + lane < p.N) ? __ldg(p.ep_ptr[k] + col0 + lane) : 0.0f;
       }
     }
@@ -539,8 +546,12 @@ struct EpilogueOut {
 #pragma unroll
       for (int k = 0; k < AB_EP_NOPS; ++k) {
         if (is_row_op(k) && sc.vec[k]) {
-#pragma unroll
-          for (int t = 0; t < 8; ++t) ev[k][t] = pre.rowv[row_slot(k)][j + t];
+          // N % 8 == 0 and 16-byte aligned rows (the fused launch's contract)
+          const bool in = col < p.N;
+          const float4 a = in ? __ldg(reinterpret_cast<const float4*>(p.ep_ptr[k] + col)) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+          const float4 b = in ? __ldg(reinterpret_cast<const float4*>(p.ep_ptr[k] + col + 4)) : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+          ev[k][0] = a.x; ev[k][1] = a.y; ev[k][2] = a.z; ev[k][3] = a.w;
+          ev[k][4] = b.x; ev[k][5] = b.y; ev[k][6] = b.z; ev[k][7] = b.w;
         } else if (sc.vec[k]) {
 #pragma unroll
           for (int t = 0; t < 8; ++t) ev[k][t] = __shfl_sync(0xffffffffu, pre.vec[k], j + t);
@@ -651,8 +662,8 @@ struct EpilogueOut {
   //           sector each, and the epilogue warps wait on the store queue;
   //   pass 2  lane c reads column c (32 LDS, one per row): the transpose that took 48 shuffles
   //           and ~130 selects, and the column sum becomes 31 adds without any shuffle.
-  // The buffer lives behind the operand ring, which gives up one of its 7 stages for it in the
-  // bf16 / tf32 kernels (the hi/lo kernels have the room anyway).
+  // The buffers (4 warps x 4 KB) live behind the tile's accumulator, at the end of the operand
+  // ring: the bf16 / tf32 ring keeps 4 stages with them (5 without), the hi/lo ring 2.
   static constexpr int kStageValue = AB_EP_COLSUM >= 0 ? AB_EP_COLSUM : (AB_EP_TPLANE >= 0 ? AB_EP_TPLANE : 0);
   static __device__ __forceinline__ uint32_t st_off(int r, int g) { return (uint32_t)(r * 32 + ((g ^ (r & 7)) << 2)); }
 #if AB_EP_STAGED
@@ -887,23 +898,33 @@ struct EpilogueOut {
 #endif
   }
   // the tile's accumulator (shared memory, see acc_off): 32 columns at a time in a rolled loop
-  // -- 32 live accumulator registers, and the body exists once
-  __device__ __forceinline__ void store_fused(uint32_t acc_base, int r, int c_local, long long row, long long n0,
-                                              int nchunks, int lane, const FusedScalars& sc) const {
+  // -- 32 live accumulator registers, and the body exists once.  The total of a half tile
+  // (fullsum_ws has one entry per 64 columns) is finished before the next half starts.  Once
+  // the last chunk's values have been consumed, the warp arrives on `acc_free`.
+  __device__ __forceinline__ void store_fused(uint32_t acc_base, int r, long long row, long long n0, int nchunks,
+                                              int lane, const FusedScalars& sc, uint64_t* acc_free) const {
     const bool live = row < p.M;
+    const int half_chunks = p.block_n >> 6;
     FF fs = {0.0f, 0.0f};
     ChunkPre pre;
     prefetch_chunk(pre, row, n0, live, sc, lane);
 #pragma unroll 1
     for (int c = 0; c < nchunks; ++c) {
       float x[32];
-      acc_ld_x32(acc_base, r, c_local + c * 32, x);
+      acc_ld_x32(acc_base, r, c * 32, x);
       const long long col0 = n0 + c * 32;
       fused_eval(x, row, col0, live, lane, sc, fs, pre);
+      if (c + 1 == nchunks) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(acc_free);
+      }
       if (c + 1 < nchunks) prefetch_chunk(pre, row, col0 + 32, live, sc, lane);
       fused_reduce(x, row, col0, lane);
+      if ((c + 1) % half_chunks == 0) {
+        finish_fullsum(fs, row, col0 + 32 - (p.block_n >> 1), lane);
+        fs = FF{0.0f, 0.0f};
+      }
     }
-    finish_fullsum(fs, row, n0, lane);
   }
 #endif  // AB_EPILOGUE
 };
@@ -926,7 +947,7 @@ struct EpilogueOut {
   const int kb_end = min(kb_begin + p.kb_per_split, p.num_k_blocks);            \
   (void)split; (void)tile_m; (void)tile_n;
 
-// one k-block of the consumer warpgroup: 4 K steps of 32 bytes, 3 products each for the
+// one k-block of an MMA warpgroup: 4 K steps of 32 bytes, 3 products each for the
 // hi/lo split (small cross terms first, the dominant hi*hi term last)
 template <int KIND, int TA, int TB>
 __device__ __forceinline__ void mma_kblock(float (&d)[64], int nparts, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
@@ -952,7 +973,7 @@ __device__ __forceinline__ void mma_kblock(float (&d)[64], int nparts, uint32_t 
 // one (CL * 128) x 128 tile; they share the B tile, each CTA loading 1/CL of it and multicasting
 // that part into the shared memory of all CL CTAs (cp.async.bulk.tensor ... multicast::cluster).
 // A ring stage of a CTA is then written by every CTA of the cluster, so it is free only when the
-// consumers of all of them have released it: every consumer warp arrives on the empty barrier of
+// MMA warpgroups of all of them have released it: every MMA warp arrives on the empty barrier of
 // every CTA (count 8 * CL).  The arithmetic per output element is the single-CTA kernel's.
 template <int CL>
 __device__ __forceinline__ void release_stage(uint64_t* bar) {
@@ -989,6 +1010,8 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
                                              ~static_cast<uintptr_t>(1023));
   __shared__ __align__(8) uint64_t full_bar[8];
   __shared__ __align__(8) uint64_t empty_bar[8];
+  __shared__ __align__(8) uint64_t acc_full;   // the shared accumulator holds a finished unit
+  __shared__ __align__(8) uint64_t acc_empty;  // ... and has been read by the epilogue
 
   const int warp = threadIdx.x >> 5;
   const int stage_bytes = p.stage_bytes;
@@ -1003,15 +1026,17 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], CL * kEpiThreads / 32);  // one arrival per consumer warp (of each CTA)
+      mbar_init(&empty_bar[s], CL * kMmaThreads / 32);  // one arrival per MMA warp (of each CTA)
     }
+    mbar_init(&acc_full, kMmaThreads / 32);
+    mbar_init(&acc_empty, kEpiThreads / 32);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
   __syncthreads();
   if (CL > 1) cluster_sync_all();  // every CTA's barriers exist before any multicast or remote arrive
 
-  if (warp < kEpiWarp0) {
+  if (warp < kMmaWarp0) {
     AB_SETMAXNREG_CONTROL(CL);
     if (warp == 0 && elect_one()) {
       // ================= TMA producer =================
@@ -1048,27 +1073,21 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
         }
       }
     }
-  } else {
-    AB_SETMAXNREG_EPILOGUE(CL);
-    // ================= consumers: wgmma, then the epilogue (warps 4..11) =================
-    const int cw = (warp - kEpiWarp0) >> 2;  // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+  } else if (warp < kEpiWarp0) {
+    AB_SETMAXNREG_MMA(CL);
+    // ================= MMA warpgroups (warps 4..11) =================
+    const int cw = (warp - kMmaWarp0) >> 2;  // tile rows [64 cw, 64 cw + 64)
     uint32_t lane_reg;
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane_reg));
     const int lane = (int)lane_reg;
     const int mma_row0 = 64 * cw + 16 * (warp & 3);  // first accumulator row of this warp's fragment
-    // epilogue: two warps per 32-row quarter, each owns half of the tile's columns
-    const int q = warp & 3;
-    const int half = cw;
-    const int half_n = p.block_n >> 1;
-    const int nchunks = half_n >> 5;
-    // the operand layout is read from the kernel parameter where it is used, not held in
-    // registers across the epilogue (which needs all of them in the larger fused regions)
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, acc_phase = 0;
     for (long long unit = group; unit < p.num_units; unit += n_groups) {
       AB_UNIT_DECODE
-      // the shared accumulator is free once every consumer has finished the previous tile's epilogue
-      asm volatile("bar.sync 2, %0;" ::"r"(kEpiThreads) : "memory");
+      float tot[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) tot[i] = -0.0f;
       for (int kb0 = kb_begin; kb0 < kb_end; kb0 += p.seg_kblocks) {
         const int kb1 = min(kb0 + p.seg_kblocks, kb_end);
         float d[64];
@@ -1103,29 +1122,53 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
         }
         wgmma_wait<0>();
         if (lane == 0) release_stage<CL>(&empty_bar[prev]);
-        acc_fold(acc_base, d, mma_row0, lane, kb0 == kb_begin);
+        acc_fold(tot, d);
       }
-      asm volatile("bar.sync 2, %0;" ::"r"(kEpiThreads) : "memory");  // the tile's accumulator is complete
+      // the shared accumulator is free once the epilogue warps have read the previous unit
+      // (parity 1 of the fresh barrier counts as complete: the first unit does not wait)
+      mbar_wait(&acc_empty, acc_phase ^ 1);
+      acc_phase ^= 1;
+      acc_store(acc_base, tot, mma_row0, lane);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&acc_full);
+    }
+  } else {
+    AB_SETMAXNREG_EPILOGUE(CL);
+    // ================= epilogue warpgroup (warps 12..15) =================
+    uint32_t lane_reg;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane_reg));
+    const int lane = (int)lane_reg;
+    const int q = warp & 3;       // tile rows [32 q, 32 q + 32), one per lane
+    const int r = q * 32 + lane;
+    uint32_t acc_phase = 0;
+    for (long long unit = group; unit < p.num_units; unit += n_groups) {
+      AB_UNIT_DECODE
       const long long m0 = tile_m * (CL * BLOCK_M) + (long long)crank * BLOCK_M;
-      const long long n0 = tile_n * p.block_n + half * half_n;
-      const int r = q * 32 + lane;
-      // built per tile: held across the main loop, the epilogue's state would cost the larger
+      const long long n0 = tile_n * p.block_n;
+      // built per tile: held across the wait, the epilogue's state would cost the larger
       // generated regions their registers
 #if AB_EP_STAGED
-      const EpilogueOut eo(p, acc_base + kAccBytes + (uint32_t)((warp - kEpiWarp0) * kStageBytesPerWarp));
+      const EpilogueOut eo(p, acc_base + kAccBytes + (uint32_t)(q * kStageBytesPerWarp));
 #else
       const EpilogueOut eo(p);
 #endif
+      mbar_wait(&acc_full, acc_phase);
+      acc_phase ^= 1;
 #ifdef AB_EPILOGUE
       const EpilogueOut::FusedScalars sc = eo.load_scalars();  // the region's [1, 1] operands
-      eo.store_fused(acc_base, r, half * half_n, m0 + r, n0, nchunks, lane, sc);  // fused launches are never split along K
+      eo.store_fused(acc_base, r, m0 + r, n0, p.block_n >> 5, lane, sc, &acc_empty);  // fused launches are never split along K
 #else
-      float acc[kAccRegs];
+#pragma unroll 1
+      for (int h = 0; h < BLOCK_N / kAccRegs; ++h) {
+        float acc[kAccRegs];
 #pragma unroll
-      for (int c = 0; c < kAccRegs / 32; ++c)
-        acc_ld_x32(acc_base, r, half * half_n + c * 32, *reinterpret_cast<float(*)[32]>(&acc[c * 32]));
-      if (split == 0) eo.store(acc, m0 + r, n0, nchunks);
-      else eo.store_partial(acc, m0 + r, n0, nchunks, split);
+        for (int c = 0; c < kAccRegs / 32; ++c)
+          acc_ld_x32(acc_base, r, h * kAccRegs + c * 32, *reinterpret_cast<float(*)[32]>(&acc[c * 32]));
+        if (split == 0) eo.store(acc, m0 + r, n0 + h * kAccRegs, kAccRegs / 32);
+        else eo.store_partial(acc, m0 + r, n0 + h * kAccRegs, kAccRegs / 32, split);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&acc_empty);
 #endif
     }
   }

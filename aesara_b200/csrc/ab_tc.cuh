@@ -21,9 +21,10 @@ namespace tc {
 
 constexpr int BLOCK_M = 128;
 constexpr int SW_BYTES = 128;  // swizzle span = smem row pitch of every operand tile
-// three warpgroups: {TMA warp, three idle warps} hand most of their registers (setmaxnreg) to
-// the two consumer warpgroups, which issue the wgmma of 64 tile rows each and run the epilogue
-constexpr int kThreads = 384;
+// four warpgroups of the GEMM: {TMA warp, three idle warps} hand most of their registers
+// (setmaxnreg) to the two MMA warpgroups, which issue the wgmma of 64 tile rows each, and to
+// the epilogue warpgroup, which stores one tile while the MMA warpgroups compute the next
+constexpr int kThreads = 512;
 constexpr int kMaxSmemGemm = 226 * 1024;   // dynamic shared memory asked for (227 KB is the per-block limit)
 
 // ----------------------------------------------------------------------------- PTX
