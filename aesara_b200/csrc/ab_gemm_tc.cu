@@ -647,8 +647,12 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     return splitk_finish(p, st);
   }
   if (ep) {
+    // one entry point per MMA-loop layout (ab_gemm_tc_kernel.cuh, AB_EP_KERNEL)
+    static const char* const f16_names[4] = {"ab_gemm_ep_f16", "ab_gemm_ep_f16_km", "ab_gemm_ep_f16_mk",
+                                             "ab_gemm_ep_f16_mm"};
+    const char* name = bf16 ? f16_names[2 * p.a_mn + p.b_mn] : (parts == 2 ? "ab_gemm_ep_tf32" : "ab_gemm_ep_tf32_1p");
     cudaKernel_t kern;
-    if ((rc = fused_kernel(ep->module, bf16 ? "ab_gemm_ep_f16" : "ab_gemm_ep_tf32", &kern))) return rc;
+    if ((rc = fused_kernel(ep->module, name, &kern))) return rc;
     void* args[] = {&ma[0], &ma[1], &mb[0], &mb[1], &p};
     AB_CUDA(cudaLaunchKernel((const void*)kern, grid, dim3(kThreads), args, smem, st));
     g_launches++;

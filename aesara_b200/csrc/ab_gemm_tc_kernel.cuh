@@ -948,9 +948,9 @@ struct EpilogueOut {
   (void)split; (void)tile_m; (void)tile_n;
 
 // one k-block of an MMA warpgroup: 4 K steps of 32 bytes, 3 products each for the
-// hi/lo split (small cross terms first, the dominant hi*hi term last)
-template <int KIND, int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float (&d)[64], int nparts, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+// hi/lo split (NP == 2: small cross terms first, the dominant hi*hi term last)
+template <int KIND, int TA, int TB, int NP>
+__device__ __forceinline__ void mma_kblock(float (&d)[64], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                            uint32_t b_lo, uint32_t a_kstep, uint32_t b_kstep, uint32_t a_lbo,
                                            uint32_t b_lbo, bool fresh) {
 #pragma unroll
@@ -959,7 +959,7 @@ __device__ __forceinline__ void mma_kblock(float (&d)[64], int nparts, uint32_t 
     const uint32_t acc = (!fresh || k > 0) ? 1u : 0u;
     if (KIND == 1) {
       wgmma_m64n128k16_bf16<TA, TB>(d, make_smem_desc(a_hi + ka, a_lbo), make_smem_desc(b_hi + kb_off, b_lbo), acc);
-    } else if (nparts == 2) {
+    } else if (NP == 2) {
       wgmma_m64n128k8_tf32(d, make_smem_desc(a_lo + ka, a_lbo), make_smem_desc(b_hi + kb_off, b_lbo), acc);
       wgmma_m64n128k8_tf32(d, make_smem_desc(a_hi + ka, a_lbo), make_smem_desc(b_lo + kb_off, b_lbo), 1u);
       wgmma_m64n128k8_tf32(d, make_smem_desc(a_hi + ka, a_lbo), make_smem_desc(b_hi + kb_off, b_lbo), 1u);
@@ -1000,7 +1000,82 @@ __device__ __forceinline__ void load_b_part(uint8_t* dst, const CUtensorMap* map
   }
 }
 
-template <int KIND, int CL = 1>
+// The MMA warpgroups' unit loop for ONE operand layout, fixed at compile time: TA / TB = 1 for an
+// MN-major A / B (bf16 only), NP = 2 for the hi/lo split.  gemm_body picks the instantiation
+// once, before the loop.  A layout chosen by a branch around each k-block's wgmmas cost the
+// pipelining: ptxas closes a wgmma group at the end of each branch (warning C7519), the commit
+// after the join then commits an empty group, and wait_group 1 waits for the real k-block.
+// The accumulator d is declared once, outside the segment loop, and nothing but wgmma writes it
+// between the fence and the wait: a fresh segment starts with scale-d = 0 on its first wgmma,
+// and acc_fold reads d only after wait_group 0.  So wait_group 1 keeps the previous k-block in
+// flight, and the only full waits are the segment drains.  Every field of p the loop reads is
+// copied into a local before it (see OperandLoad).
+template <int KIND, int TA, int TB, int NP, int CL>
+__device__ __forceinline__ void mma_loop(const GemmParams& p, uint32_t ring, uint64_t* full_bar, uint64_t* empty_bar,
+                                         uint64_t* acc_full, uint64_t* acc_empty, uint32_t acc_base,
+                                         long long group, long long n_groups, int cw, int lane, int mma_row0) {
+  const long long num_units = p.num_units, num_tiles = p.num_tiles;
+  const int kb_per_split = p.kb_per_split, num_k_blocks = p.num_k_blocks, seg_kblocks = p.seg_kblocks;
+  const int stages = p.stages;
+  const uint32_t stage_bytes = (uint32_t)p.stage_bytes;
+  const uint32_t a_tile_bytes = (uint32_t)p.a_tile_bytes, b_tile_bytes = (uint32_t)p.b_tile_bytes;
+  const uint32_t chunk_bytes = (uint32_t)p.chunk_bytes;
+  const uint32_t a_kstep = (uint32_t)p.a_kstep, b_kstep = (uint32_t)p.b_kstep;
+  const uint32_t a_lbo = TA ? chunk_bytes : 16u, b_lbo = TB ? chunk_bytes : 16u;
+  // this warpgroup's 64 rows of the A tile: 64 K-major rows of 128 B, or MN chunk cw
+  const uint32_t a_off = TA ? (uint32_t)cw * chunk_bytes : (uint32_t)(cw * 64 * SW_BYTES);
+  const uint32_t b_off = NP * a_tile_bytes;
+  float d[64], tot[64];
+  // Defined once, before any wgmma: a segment's first wgmma ignores d (scale-d = 0), but the
+  // CUDA 12.8 ptxas (NVRTC as bundled with PyTorch) counts an undefined accumulator input as a
+  // non-wgmma definition inside the pipeline stage and serialises every wgmma of the kernel
+  // (C7515: one wait_group 0 after each).
+#pragma unroll
+  for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+  int stage = 0;
+  uint32_t phase = 0, acc_phase = 0;
+  for (long long unit = group; unit < num_units; unit += n_groups) {
+    const int split = (int)(unit / num_tiles);  // the K range of the unit (AB_UNIT_DECODE)
+    const int kb_begin = split * kb_per_split;
+    const int kb_end = min(kb_begin + kb_per_split, num_k_blocks);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) tot[i] = -0.0f;
+    for (int kb0 = kb_begin; kb0 < kb_end; kb0 += seg_kblocks) {
+      const int kb1 = min(kb0 + seg_kblocks, kb_end);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sbase = ring + (uint32_t)stage * stage_bytes;
+        const uint32_t a_hi = sbase + a_off, b_hi = sbase + b_off;
+        wgmma_fence();
+        mma_kblock<KIND, TA, TB, NP>(d, a_hi, a_hi + a_tile_bytes, b_hi, b_hi + b_tile_bytes, a_kstep, b_kstep,
+                                     a_lbo, b_lbo, kb == kb0);
+        wgmma_commit();
+        // the previous k-block's products have retired: its stage goes back to the producer
+        wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) release_stage<CL>(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == stages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (lane == 0) release_stage<CL>(&empty_bar[prev]);
+      acc_fold(tot, d);
+    }
+    // the shared accumulator is free once the epilogue warps have read the previous unit
+    // (parity 1 of the fresh barrier counts as complete: the first unit does not wait)
+    mbar_wait(acc_empty, acc_phase ^ 1);
+    acc_phase ^= 1;
+    acc_store(acc_base, tot, mma_row0, lane);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(acc_full);
+  }
+}
+
+// LAYOUT: the MMA loop's layout, fixed by the kernel -- 2 * a_mn + b_mn for KIND 1, nparts for
+// KIND 0 -- or -1: chosen from p at run time, once, before the unit loop (the ahead-of-time
+// kernels).  The NVRTC build has one entry point per layout instead: with the four bf16 loops in
+// one kernel, the CUDA 12.8 ptxas spills in the larger epilogue regions (560-byte stack frame).
+template <int KIND, int CL = 1, int LAYOUT = -1>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUtensorMap& map_a1,
                                           const CUtensorMap& map_b0, const CUtensorMap& map_b1,
                                           const GemmParams& p) {
@@ -1081,57 +1156,24 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
     asm volatile("mov.u32 %0, %%laneid;" : "=r"(lane_reg));
     const int lane = (int)lane_reg;
     const int mma_row0 = 64 * cw + 16 * (warp & 3);  // first accumulator row of this warp's fragment
-    int stage = 0;
-    uint32_t phase = 0, acc_phase = 0;
-    for (long long unit = group; unit < p.num_units; unit += n_groups) {
-      AB_UNIT_DECODE
-      float tot[64];
-#pragma unroll
-      for (int i = 0; i < 64; ++i) tot[i] = -0.0f;
-      for (int kb0 = kb_begin; kb0 < kb_end; kb0 += p.seg_kblocks) {
-        const int kb1 = min(kb0 + p.seg_kblocks, kb_end);
-        float d[64];
-        int prev = -1;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t sbase = smem_u32(smem + (size_t)stage * p.stage_bytes);
-          // this warpgroup's 64 rows of the A tile: 64 K-major rows of 128 B, or MN chunk cw
-          const uint32_t a_hi = sbase + (p.a_mn ? (uint32_t)(cw * p.chunk_bytes) : (uint32_t)(cw * 64 * SW_BYTES));
-          const uint32_t a_lo = a_hi + (uint32_t)p.a_tile_bytes;
-          const uint32_t b_hi = sbase + (uint32_t)(p.nparts * p.a_tile_bytes);
-          const uint32_t b_lo = b_hi + (uint32_t)p.b_tile_bytes;
-          const uint32_t a_lbo = p.a_mn ? (uint32_t)p.chunk_bytes : 16u;
-          const uint32_t b_lbo = p.b_mn ? (uint32_t)p.chunk_bytes : 16u;
-          const uint32_t a_kstep = (uint32_t)p.a_kstep, b_kstep = (uint32_t)p.b_kstep;
-          wgmma_fence();
-          if (KIND == 0) {
-            mma_kblock<0, 0, 0>(d, p.nparts, a_hi, a_lo, b_hi, b_lo, a_kstep, b_kstep, a_lbo, b_lbo, kb == kb0);
-          } else if (p.a_mn) {
-            if (p.b_mn) mma_kblock<1, 1, 1>(d, 1, a_hi, a_lo, b_hi, b_lo, a_kstep, b_kstep, a_lbo, b_lbo, kb == kb0);
-            else mma_kblock<1, 1, 0>(d, 1, a_hi, a_lo, b_hi, b_lo, a_kstep, b_kstep, a_lbo, b_lbo, kb == kb0);
-          } else {
-            if (p.b_mn) mma_kblock<1, 0, 1>(d, 1, a_hi, a_lo, b_hi, b_lo, a_kstep, b_kstep, a_lbo, b_lbo, kb == kb0);
-            else mma_kblock<1, 0, 0>(d, 1, a_hi, a_lo, b_hi, b_lo, a_kstep, b_kstep, a_lbo, b_lbo, kb == kb0);
-          }
-          wgmma_commit();
-          // the previous k-block's products have retired: its stage goes back to the producer
-          wgmma_wait<1>();
-          if (prev >= 0 && lane == 0) release_stage<CL>(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        wgmma_wait<0>();
-        if (lane == 0) release_stage<CL>(&empty_bar[prev]);
-        acc_fold(tot, d);
-      }
-      // the shared accumulator is free once the epilogue warps have read the previous unit
-      // (parity 1 of the fresh barrier counts as complete: the first unit does not wait)
-      mbar_wait(&acc_empty, acc_phase ^ 1);
-      acc_phase ^= 1;
-      acc_store(acc_base, tot, mma_row0, lane);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_full);
+    const uint32_t ring = smem_u32(smem);
+#define AB_MMA_LOOP(TA, TB, NP)                                                                          \
+  mma_loop<KIND, TA, TB, NP, CL>(p, ring, full_bar, empty_bar, &acc_full, &acc_empty, acc_base, group, n_groups, \
+                                 cw, lane, mma_row0)
+    if constexpr (LAYOUT >= 0) {
+      if constexpr (KIND == 0) AB_MMA_LOOP(0, 0, LAYOUT == 1 ? 1 : 2);
+      else AB_MMA_LOOP((LAYOUT >> 1) & 1, LAYOUT & 1, 1);
+    } else if (KIND == 0) {  // tf32 operands are always K-major (plan_operand)
+      if (p.nparts == 2) AB_MMA_LOOP(0, 0, 2);
+      else AB_MMA_LOOP(0, 0, 1);
+    } else if (p.a_mn) {
+      if (p.b_mn) AB_MMA_LOOP(1, 1, 1);
+      else AB_MMA_LOOP(1, 0, 1);
+    } else {
+      if (p.b_mn) AB_MMA_LOOP(0, 1, 1);
+      else AB_MMA_LOOP(0, 0, 1);
     }
+#undef AB_MMA_LOOP
   } else {
     AB_SETMAXNREG_EPILOGUE(CL);
     // ================= epilogue warpgroup (warps 12..15) =================
@@ -1179,13 +1221,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
 extern "C" __global__ void ab_gemm_ep_staged_marker() {}  // tells gemm_run to reserve kStageBytes
 #endif
 #ifdef AB_EPILOGUE
-// NVRTC build: C-linkage entry points (the module is loaded by name from gemm_run)
-extern "C" __global__ void __launch_bounds__(kGemmThreads, 1)
-ab_gemm_ep_tf32(const __grid_constant__ CUtensorMap a0, const __grid_constant__ CUtensorMap a1,
-                const __grid_constant__ CUtensorMap b0, const __grid_constant__ CUtensorMap b1,
-                const __grid_constant__ GemmParams p) { gemm_body<0>(a0, a1, b0, b1, p); }
-extern "C" __global__ void __launch_bounds__(kGemmThreads, 1)
-ab_gemm_ep_f16(const __grid_constant__ CUtensorMap a0, const __grid_constant__ CUtensorMap a1,
-               const __grid_constant__ CUtensorMap b0, const __grid_constant__ CUtensorMap b1,
-               const __grid_constant__ GemmParams p) { gemm_body<1>(a0, a1, b0, b1, p); }
+// NVRTC build: C-linkage entry points, one per MMA-loop layout (the module is loaded by name
+// from gemm_run, which picks the kernel of the packed operands' layout)
+#define AB_EP_KERNEL(NAME, KIND, LAYOUT)                                                               \
+  extern "C" __global__ void __launch_bounds__(kGemmThreads, 1)                                       \
+  NAME(const __grid_constant__ CUtensorMap a0, const __grid_constant__ CUtensorMap a1,                 \
+       const __grid_constant__ CUtensorMap b0, const __grid_constant__ CUtensorMap b1,                 \
+       const __grid_constant__ GemmParams p) { gemm_body<KIND, 1, LAYOUT>(a0, a1, b0, b1, p); }
+AB_EP_KERNEL(ab_gemm_ep_tf32, 0, 2)     // 3xTF32: hi/lo planes
+AB_EP_KERNEL(ab_gemm_ep_tf32_1p, 0, 1)  // one TF32 pass
+AB_EP_KERNEL(ab_gemm_ep_f16, 1, 0)      // bf16, A and B K-major
+AB_EP_KERNEL(ab_gemm_ep_f16_km, 1, 1)   // bf16, B MN-major
+AB_EP_KERNEL(ab_gemm_ep_f16_mk, 1, 2)   // bf16, A MN-major
+AB_EP_KERNEL(ab_gemm_ep_f16_mm, 1, 3)   // bf16, A and B MN-major
+#undef AB_EP_KERNEL
 #endif

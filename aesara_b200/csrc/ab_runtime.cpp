@@ -194,6 +194,13 @@ int ab_nvrtc_compile(const char* src, const char* name, const char* const* extra
   return AB_OK;
 }
 
+int ab_nvrtc_version(int* major, int* minor) {
+  if (!major || !minor) return fail(AB_ERR_INVALID, "null argument");
+  nvrtcResult r = nvrtcVersion(major, minor);
+  if (r != NVRTC_SUCCESS) return fail(AB_ERR_NVRTC, "nvrtcVersion: %s", nvrtcGetErrorString(r));
+  return AB_OK;
+}
+
 void ab_buffer_free(void* p) { free(p); }
 
 int ab_module_load(const void* cubin, size_t cubin_size, ab_module** out) {

@@ -60,6 +60,7 @@ SIGNATURES = {
         C.c_int,
         [C.c_char_p, C.c_char_p, C.POINTER(C.c_char_p), C.c_int, c_voidpp, C.POINTER(C.c_size_t)],
     ),
+    "ab_nvrtc_version": (C.c_int, [c_i32p, c_i32p]),
     "ab_buffer_free": (None, [C.c_void_p]),
     "ab_module_load": (C.c_int, [C.c_void_p, C.c_size_t, c_voidpp]),
     "ab_module_unload": (C.c_int, [C.c_void_p]),
@@ -288,10 +289,21 @@ def _find_cache_dir(d):
     return d
 
 
+def nvrtc_version() -> tuple:
+    """(major, minor) of the NVRTC that compiles the generated kernels: the libnvrtc.so.12
+    loaded first in this process (torch's bundled one once torch is imported)."""
+    major, minor = C.c_int32(), C.c_int32()
+    check(load().ab_nvrtc_version(C.byref(major), C.byref(minor)))
+    return major.value, minor.value
+
+
 def compile_cubin(src: str, name: str = "ab_module") -> bytes:
-    """NVRTC-compile ``src`` for sm_90a (disk-cached).  Needs no GPU."""
+    """NVRTC-compile ``src`` for sm_90a (disk-cached).  Needs no GPU.  The cache key holds the
+    library version and the NVRTC version: two NVRTC versions make different code from one
+    source."""
     lib = load()
-    key = hashlib.sha256((lib.ab_version().decode() + src).encode()).hexdigest()[:40]
+    nvrtc = "nvrtc %d.%d\n" % nvrtc_version()
+    key = hashlib.sha256((lib.ab_version().decode() + nvrtc + src).encode()).hexdigest()[:40]
     path = os.path.join(cache_dir(), f"{name}_{key}.cubin")
     if os.path.exists(path):
         try:

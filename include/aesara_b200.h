@@ -88,6 +88,10 @@ int ab_event_destroy(void* ev);
  * malloc()ed; release with ab_buffer_free. */
 int ab_nvrtc_compile(const char* src, const char* name, const char* const* extra_opts,
                      int n_extra_opts, void** cubin, size_t* cubin_size);
+/* Version of the NVRTC that ab_nvrtc_compile uses: the libnvrtc.so.12 the process loaded
+ * first (a process that has imported torch uses torch's bundled one).  Part of the key of
+ * the cubin cache, since two NVRTC versions make different code from the same source. */
+int ab_nvrtc_version(int* major, int* minor);
 void ab_buffer_free(void* p);
 /* Load a cubin on the current device (replaces dlimport of the compiled module,
  * aesara/link/c/cmodule.py:ModuleCache). */
