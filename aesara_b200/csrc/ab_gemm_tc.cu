@@ -85,13 +85,7 @@ pack_rows_kernel(const float* __restrict__ in, long long R, long long Kc, long l
     } else {
       float hi[8], lo[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        uint32_t hb, lb;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v[j]));
-        hi[j] = __uint_as_float(hb);
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(v[j] - hi[j]));
-        lo[j] = __uint_as_float(lb);
-      }
+      for (int j = 0; j < 8; ++j) tf32_split(v[j], hi[j], lo[j]);
       float* oh = static_cast<float*>(out0) + r * pitch + c;
       float* ol = static_cast<float*>(out1) + r * pitch + c;
       *reinterpret_cast<float4*>(oh) = make_float4(hi[0], hi[1], hi[2], hi[3]);
@@ -125,13 +119,10 @@ pack_kernel(const float* __restrict__ in, long long R, long long Kc, long long s
     if (r < R && c < Kc) {
       const float v = tile[ty + i][tx];
       if (MODE == 0) {
-        uint32_t hi_bits, lo_bits;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi_bits) : "f"(v));
-        const float hi = __uint_as_float(hi_bits);
-        const float lo = v - hi;
-        asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo_bits) : "f"(lo));
+        float hi, lo;
+        tf32_split(v, hi, lo);
         static_cast<float*>(out0)[r * pitch + c] = hi;
-        static_cast<float*>(out1)[r * pitch + c] = __uint_as_float(lo_bits);
+        static_cast<float*>(out1)[r * pitch + c] = lo;
       } else if (MODE == 1) {
         static_cast<float*>(out0)[r * pitch + c] = v;
       } else {

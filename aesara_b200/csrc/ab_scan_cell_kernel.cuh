@@ -235,13 +235,7 @@ __device__ __forceinline__ void cell_scan_body(const CUtensorMap& map_h00, const
                 // the state that feeds the next step's Gemm, also as its hi/lo TF32 planes
                 float hh[2], hl[2];
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  uint32_t hb, lb;
-                  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(ov[k][e]));
-                  hh[e] = __uint_as_float(hb);
-                  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(ov[k][e] - hh[e]));
-                  hl[e] = __uint_as_float(lb);
-                }
+                for (int e = 0; e < 2; ++e) tf32_split(ov[k][e], hh[e], hl[e]);
                 *reinterpret_cast<float2*>(hp_hi + so) = make_float2(hh[0], hh[1]);
                 *reinterpret_cast<float2*>(hp_lo + so) = make_float2(hl[0], hl[1]);
               }

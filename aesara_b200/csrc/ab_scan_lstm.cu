@@ -80,13 +80,10 @@ split_planes_kernel(const float* __restrict__ src, long long R, long long K, lon
     const long long gate = rem / CELL_UNITS, u = rem % CELL_UNITS;
     rs = gate * interleave_h + tile * CELL_UNITS + u;
   }
-  const float v = src[rs * s_r + k * s_k];
-  uint32_t hb, lb;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v));
-  const float h = __uint_as_float(hb);
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(v - h));
+  float h, l;
+  tf32_split(src[rs * s_r + k * s_k], h, l);
   hi[i] = h;
-  lo[i] = __uint_as_float(lb);
+  lo[i] = l;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,

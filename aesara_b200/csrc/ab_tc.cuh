@@ -203,6 +203,20 @@ __device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t a_d
       : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
+// 3xTF32 split: hi = tf32(v) rounded to nearest (ties away), lo = tf32(v - hi).  cvt.rna rounds a
+// finite v whose magnitude's bit pattern is at or above 0x7F7FF000 (halfway between the largest
+// TF32 value and 2^128) up to Inf, and hi = Inf, lo = -Inf would make every product with v NaN
+// where sgemm is finite.  Such a v takes the truncated value as hi instead; v - hi is then exact
+// and lo stays finite.  Used by every hi/lo pack: GEMM operands, Scan weights and Scan states.
+__device__ __forceinline__ void tf32_split(float v, float& hi, float& lo) {
+  uint32_t hb, lb;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hb) : "f"(v));
+  const uint32_t vb = __float_as_uint(v);
+  if ((hb & 0x7FFFFFFFu) == 0x7F800000u && (vb & 0x7FFFFFFFu) < 0x7F800000u) hb = vb & 0xFFFFE000u;
+  hi = __uint_as_float(hb);
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lb) : "f"(v - hi));
+  lo = __uint_as_float(lb);
+}
 
 }  // namespace tc
 }  // namespace ab

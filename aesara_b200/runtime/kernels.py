@@ -2,6 +2,7 @@
 
 from __future__ import annotations
 
+import collections
 import ctypes as C
 import os
 
@@ -367,6 +368,12 @@ class PackCache:
         return _lib.GemmOperand(p0, p1, rows, k, pitch, mn, precision)
 
 
+# tensor-core GEMM launches made through ``gemm``, keyed by (fused, precision, a_mn, b_mn): the
+# operand layouts select the MMA loop (ahead-of-time kernels) or the entry point (fused modules),
+# so tests can tell which of them ran.  CUDA-graph replays do not pass through here.
+TC_LAUNCHES = collections.Counter()
+
+
 def gemm(C_: DeviceArray, alpha, A: DeviceArray, B: DeviceArray, beta, precision=0, cache=None,
          cin: DeviceArray = None, epilogue=None):
     """C <- beta*Cin + alpha*A@B (Cin = C, i.e. in place, unless ``cin`` is given).
@@ -380,6 +387,7 @@ def gemm(C_: DeviceArray, alpha, A: DeviceArray, B: DeviceArray, beta, precision
         cache = cache if cache is not None else PackCache()
         opa = cache.operand(A, m, k, A.strides[0], A.strides[1], precision)
         opb = cache.operand(B, n, k, B.strides[1], B.strides[0], precision)
+        TC_LAUNCHES[(epilogue is not None, precision, opa.mn_major, opb.mn_major)] += 1
         cin_args = (None, 0, 0) if cin is None else (cin.ptr, cin.strides[0], cin.strides[1])
         if epilogue is not None:
             ep = _lib.GemmEpilogue()

@@ -4,7 +4,7 @@ integer/bool outputs, rtol 1e-5 for floats (see tests/_cases.py)."""
 import numpy as np
 import pytest
 
-from tests._cases import assert_matches, case_names, load_case, uses_blas
+from tests._cases import assert_matches, case_names, fused_vs_plain, load_case, mlp_inputs, mlp_truth, uses_blas
 
 pytestmark = pytest.mark.gpu
 
@@ -235,12 +235,7 @@ def test_mlp_medium_size_fp32_faithful_vs_oracle(rt):
            (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), np.zeros(H, "float32"),
            (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), np.zeros(H, "float32")]
     cpu32 = run_program(prog, [np.array(a) for a in ins])
-    X, Y, W1, b1, W2, b2 = [a.astype(np.float64) for a in ins]
-    h = np.tanh(X @ W1 + b1)
-    diff = h @ W2 + b2 - Y
-    dout = 2.0 * diff / diff.size
-    dpre = (dout @ W2.T) * (1.0 - h * h)
-    truth = [np.mean(diff ** 2), X.T @ dpre, dpre.sum(0), h.T @ dout, dout.sum(0)]
+    truth = mlp_truth(ins)
 
     def nerr(a, t):
         return float(np.max(np.abs(np.asarray(a, np.float64) - t)) / max(np.max(np.abs(t)), 1e-300))
@@ -261,25 +256,6 @@ def lib_launches():
     return lib.load().ab_launch_count()
 
 
-def _fused_vs_plain(fused, plain, what, exact_sums=True):
-    """cfg3 outputs [loss, dW1, db1, dW2, db2]: the products see identical operands (the
-    epilogue evaluates the same scalar expressions on the same fp32 values; a bf16 plane written
-    by the epilogue equals the separate pack), so the weight gradients are BIT-identical.  Loss
-    and bias gradients, fp32-faithful policy: float64(-equivalent) sums of identical float32
-    terms in a different (still deterministic) order: equal to the last float32 bit or one ulp.
-    tf32 / bf16 policies (``exact_sums=False``): the epilogue adds 8 / 32 terms at a time as a
-    float32 tree before the float64 stage -- a few 2^-24 of the sum of magnitudes, checked
-    norm-wise at 2e-6 (the terms themselves carry 2^-8 from the bf16 operands)."""
-    for k, (a, b) in enumerate(zip(fused, plain)):
-        if np.ndim(a) == 2:
-            np.testing.assert_array_equal(a, b, err_msg=f"{what} output {k}: fused vs node-by-node")
-        elif exact_sums:
-            np.testing.assert_allclose(a, b, rtol=3e-7, atol=0, err_msg=f"{what} output {k}: fused vs node-by-node")
-        else:
-            np.testing.assert_allclose(a, b, rtol=0, atol=2e-6 * float(np.max(np.abs(b))),
-                                       err_msg=f"{what} output {k}: fused vs node-by-node")
-
-
 @pytest.mark.parametrize("precision", [0, 2])
 def test_mlp_gemm_epilogue_fusion_matches_node_by_node(rt, precision, monkeypatch):
     """cfg3 graph, B=1024, H=512: the three Gemm/Dot22 -> Elemwise pairs run as fused
@@ -295,9 +271,7 @@ def test_mlp_gemm_epilogue_fusion_matches_node_by_node(rt, precision, monkeypatc
         monkeypatch.setenv("AB_GEMM_FUSE_FP32", "1")
     rng = np.random.default_rng(21)
     B, H = 1024, 512
-    ins = [rng.standard_normal((B, H)).astype("float32"), rng.standard_normal((B, H)).astype("float32"),
-           (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), (rng.standard_normal(H) * 0.1).astype("float32"),
-           (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), (rng.standard_normal(H) * 0.1).astype("float32")]
+    ins = mlp_inputs(rng, B, H)
     ex = rt(prog, precision=precision)
     n_gemm_fusions = sum(type(f).__name__ == "GemmEpilogueFusion" for f in ex._fusions)
     assert n_gemm_fusions == 3 and len(ex._fusions) == 3  # Sqr -> Sum (the loss) is inside region 2
@@ -317,14 +291,14 @@ def test_mlp_gemm_epilogue_fusion_matches_node_by_node(rt, precision, monkeypatc
     before = lib_launches()
     plain = ex_plain(*ins)
     assert n_fused_launches < lib_launches() - before
-    _fused_vs_plain(fused, plain, f"precision {precision}", exact_sums=precision == 0)
+    fused_vs_plain(fused, plain, f"precision {precision}", exact_sums=precision == 0)
     # the round-1 regions (one Elemwise per product) still give the same bits
     os.environ["AB_GEMM_FUSE_SINGLE"] = "1"
     try:
         single = rt(prog, precision=precision)(*ins)
     finally:
         del os.environ["AB_GEMM_FUSE_SINGLE"]
-    _fused_vs_plain(single, plain, f"precision {precision}, single-node regions", exact_sums=precision == 0)
+    fused_vs_plain(single, plain, f"precision {precision}, single-node regions", exact_sums=precision == 0)
 
 
 @pytest.mark.parametrize("precision", [0, 2])
@@ -342,9 +316,7 @@ def test_mlp_gemm_epilogue_fusion_ragged_batch(rt, precision, B, monkeypatch):
         monkeypatch.setenv("AB_GEMM_FUSE_FP32", "1")
     rng = np.random.default_rng(B)
     H = 256
-    ins = [rng.standard_normal((B, H)).astype("float32"), rng.standard_normal((B, H)).astype("float32"),
-           (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), (rng.standard_normal(H) * 0.1).astype("float32"),
-           (rng.standard_normal((H, H)) / np.sqrt(H)).astype("float32"), (rng.standard_normal(H) * 0.1).astype("float32")]
+    ins = mlp_inputs(rng, B, H)
     ex = rt(prog, precision=precision)
     fused = ex(*ins)
     assert ex.fused_regions_run == 3 and not any(f.broken for f in ex._fusions)
@@ -353,7 +325,7 @@ def test_mlp_gemm_epilogue_fusion_ragged_batch(rt, precision, B, monkeypatch):
         plain = rt(prog, precision=precision)(*ins)
     finally:
         del os.environ["AB_NO_GEMM_FUSE"], os.environ["AB_NO_RED_FUSE"]
-    _fused_vs_plain(fused, plain, f"precision {precision}, B={B}", exact_sums=precision == 0)
+    fused_vs_plain(fused, plain, f"precision {precision}, B={B}", exact_sums=precision == 0)
 
 
 @pytest.mark.parametrize("T,B,H", [(12, 256, 128), (5, 384, 192), (4, 200, 64)])
@@ -485,7 +457,7 @@ def test_mlp_full_size_fused_equals_node_by_node(rt):
         plain = run(rt(prog, precision=2, host_outputs=False), X, Y)
     finally:
         del os.environ["AB_NO_GEMM_FUSE"], os.environ["AB_NO_RED_FUSE"]
-    _fused_vs_plain(fused, plain, "full-size MLP", exact_sums=False)
+    fused_vs_plain(fused, plain, "full-size MLP", exact_sums=False)
     perm = torch.randperm(B, device="cuda", generator=g)
     shuffled = run(ex, X[perm].contiguous(), Y[perm].contiguous())
     for k, (a, b) in enumerate(zip(shuffled, fused)):
@@ -617,6 +589,38 @@ def test_lstm_generated_cell_equals_the_ahead_of_time_cell(rt):
     assert [st["runner"] for st in ex2._state if "runner" in st][0].fast_path_kind == "jit"
     for a, b in zip(aot, jit):
         np.testing.assert_array_equal(a, b)
+
+
+@pytest.mark.parametrize("kind", ["lstm", "jit"])
+def test_lstm_flt_max_weight_stays_finite(rt, kind, monkeypatch):
+    """cfg4 with U[k0, j] = +-FLT_MAX, where hidden unit k0 is held at exactly 0 (all four of its
+    gate inputs are -200: i = f = o = 0, so c and h stay 0).  The float32 sgemm path gives
+    0 * FLT_MAX = 0; the persistent kernel's 3xTF32 weight planes must too.  Rounding FLT_MAX to
+    TF32 overflows to Inf, and a split of hi = Inf, lo = -Inf would make 0 * Inf = NaN in every
+    column j, on both the ahead-of-time and the generated cell."""
+    from oracle.program_np import run_program
+
+    if kind == "jit":
+        monkeypatch.setenv("AB_SCAN_JIT", "1")
+    prog, _, _ = load_case("cfg4_lstm")
+    rng = np.random.default_rng(31)
+    T, B, H = 5, 384, 128
+    k0 = 77
+    x = rng.standard_normal((T, B, 4 * H)).astype("float32")
+    x[:, :, k0::H] = -200.0
+    U = (rng.standard_normal((H, 4 * H)) / np.sqrt(H)).astype("float32")
+    U[k0, 5] = np.finfo(np.float32).max
+    U[k0, 3 * H + 9] = -np.finfo(np.float32).max
+    ins = [x, np.zeros((B, H), "float32"), np.zeros((B, H), "float32"), U]
+    with np.errstate(over="ignore"):
+        want = run_program(prog, [np.array(a) for a in ins])
+    ex = rt(prog)
+    got = ex(*ins)
+    assert [st["runner"] for st in ex._state if "runner" in st][0].fast_path_kind == kind
+    for k, (g, w) in enumerate(zip(got, want)):
+        assert np.isfinite(w).all()
+        assert np.isfinite(g).all(), f"lstm out {k}: {np.count_nonzero(~np.isfinite(g))} non-finite elements"
+        assert_matches(g, w, blas=True, rtol=1e-5, what=f"lstm out {k} with a FLT_MAX weight")
 
 
 @pytest.mark.parametrize("shape", [(1000, 777), (64, 4099), (33, 17), (5, 300, 130)])
