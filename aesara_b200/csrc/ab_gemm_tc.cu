@@ -514,12 +514,17 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     }
   }
   {
-    // Unit order inside a K range (AB_UNIT_DECODE): a tall tile grid walks groups of 8 tile
-    // rows, so that the units in flight share A and B panels in L2; a square grid keeps the
-    // plain rows-then-columns order (all column tiles of a row stream whole rows of B).
+    // Unit order inside a K range (AB_UNIT_DECODE): groups of 8 tile rows, columns outer, so
+    // that the units in flight share A and B panels in L2.  A tall tile grid always takes it;
+    // a square bf16 one once it has more tiles than the persistent grid has CTAs.  There, in
+    // row order, a wave of 132 CTAs over 32 x 32 tiles reads 5 A and 32 B panels (16 MB each
+    // at the weight gradients' K = 65536), in groups of 8 rows 8 A and 17 B panels.  Groups of
+    // 11 (11 + 12 panels) measured slower than 8 on those products, and the 3xTF32 weight
+    // gradients measured slower grouped than in row order.
     const char* gm_env = getenv("AB_GEMM_GROUP_M");  // probing knob
     const long long tm = (M + BLOCK_M - 1) / BLOCK_M, tn = (N + BLOCK_N - 1) / BLOCK_N;
-    p.group_m = gm_env ? std::max(1, atoi(gm_env)) : (tm >= 4 * tn ? 8 : 1);
+    p.group_m = (tm >= 4 * tn || (precision == 2 && tm * tn > sm_count())) ? 8 : 1;
+    if (gm_env) p.group_m = std::max(1, atoi(gm_env));
   }
   {
     // K segments (see "segments" in ab_gemm_tc_kernel.cuh): 4 k-blocks = 128 K elements for
