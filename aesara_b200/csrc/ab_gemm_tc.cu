@@ -315,17 +315,17 @@ int gemm_pack(int precision, const float* src, long long rows, long long k, long
 
 bool gemm_tc_eligible(long long M, long long N, long long K) { return eligible(M, N, K); }
 
-// CTAs per cluster of the ahead-of-time kernels: 4 (gemm_body<KIND, 4>, the B tile shared by TMA
-// multicast) when AB_GEMM_CLUSTER4 asks for it and there are at least two cluster tiles of rows;
-// 1 otherwise, and always for the fused-epilogue kernels.  Off by default: not measured faster.
-int cluster_ctas(long long M, bool fused) {
-  const bool allow = getenv("AB_GEMM_CLUSTER4") != nullptr && getenv("AB_GEMM_NO_CLUSTER4") == nullptr;
-  return (allow && !fused && M >= 2 * 4 * BLOCK_M && sm_count() % 4 == 0) ? 4 : 1;
+// CTAs per cluster: 2 (gemm_body<KIND, 2>: two CTAs stacked along M share the B tile, each
+// loading half of it by TMA multicast, so a k-block reads 24 KB from L2 per CTA instead of 32)
+// for bf16 products of at least two tile rows that are not split along K; 1 otherwise.
+// AB_GEMM_CLUSTER=1|2 forces the choice (probing knob).
+int cluster_ctas(int precision, long long M, bool fused, int k_splits) {
+  if (const char* env = getenv("AB_GEMM_CLUSTER")) return (atoi(env) == 2 && !fused) ? 2 : 1;
+  return (precision == 2 && !fused && M >= 2 * BLOCK_M && k_splits == 1) ? 2 : 1;
 }
 
-// how many clusters of `ctas` CTAs of this kernel can be resident at once (the persistent grid)
 template <typename Kern>
-int max_clusters(Kern kern, int ctas, size_t smem) {
+cudaError_t active_clusters(Kern kern, int ctas, size_t smem, int* n) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(ctas * (sm_count() / ctas)));
   cfg.blockDim = dim3(kThreads);
@@ -337,8 +337,14 @@ int max_clusters(Kern kern, int ctas, size_t smem) {
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  return cudaOccupancyMaxActiveClusters(n, kern, &cfg);
+}
+
+// how many clusters of `ctas` CTAs of this kernel can be resident at once (the persistent grid)
+template <typename Kern>
+int max_clusters(Kern kern, int ctas, size_t smem) {
   int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) {
+  if (active_clusters(kern, ctas, smem, &n) != cudaSuccess || n <= 0) {
     cudaGetLastError();
     n = sm_count() / ctas;
   }
@@ -514,19 +520,6 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     }
   }
   {
-    // Unit order inside a K range (AB_UNIT_DECODE): groups of 8 tile rows, columns outer, so
-    // that the units in flight share A and B panels in L2.  A tall tile grid always takes it;
-    // a square bf16 one once it has more tiles than the persistent grid has CTAs.  There, in
-    // row order, a wave of 132 CTAs over 32 x 32 tiles reads 5 A and 32 B panels (16 MB each
-    // at the weight gradients' K = 65536), in groups of 8 rows 8 A and 17 B panels.  Groups of
-    // 11 (11 + 12 panels) measured slower than 8 on those products, and the 3xTF32 weight
-    // gradients measured slower grouped than in row order.
-    const char* gm_env = getenv("AB_GEMM_GROUP_M");  // probing knob
-    const long long tm = (M + BLOCK_M - 1) / BLOCK_M, tn = (N + BLOCK_N - 1) / BLOCK_N;
-    p.group_m = (tm >= 4 * tn || (precision == 2 && tm * tn > sm_count())) ? 8 : 1;
-    if (gm_env) p.group_m = std::max(1, atoi(gm_env));
-  }
-  {
     // K segments (see "segments" in ab_gemm_tc_kernel.cuh): 4 k-blocks = 128 K elements for
     // the fp32-faithful mode, 16 for the others; AB_GEMM_SEG_KB overrides (0 = never fold, the
     // whole K loop stays in registers)
@@ -587,9 +580,21 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
   }
   CUtensorMap ma[2], mb[2];
   int rc;
-  // AB_GEMM_CLUSTER4=1: clusters of 4 CTAs stacked along M share the B tile by TMA multicast
-  // (gemm_body<KIND, 4>; same arithmetic, so the same result bit for bit)
-  const int cl = cluster_ctas(M, ep != nullptr);
+  // same arithmetic per output element in a pair, so the same result bit for bit
+  const int cl = cluster_ctas(precision, M, ep != nullptr, p.k_splits);
+  {
+    // Unit order inside a K range (AB_UNIT_DECODE): groups of 8 tile rows (4 pair rows),
+    // columns outer, so that the units in flight share A and B panels in L2.  A tall tile grid
+    // always takes it; a square bf16 one once it has more tiles than the persistent grid has
+    // CTAs.  There, in row order, a wave of 132 CTAs over 32 x 32 tiles reads 5 A and 32 B
+    // panels (16 MB each at the weight gradients' K = 65536), in groups of 8 rows 8 A and 17 B
+    // panels.  Groups of 11 (11 + 12 panels) measured slower than 8 on those products, and the
+    // 3xTF32 weight gradients measured slower grouped than in row order.
+    const char* gm_env = getenv("AB_GEMM_GROUP_M");  // probing knob, in rows of cluster tiles
+    const long long tm = (M + BLOCK_M - 1) / BLOCK_M, tn = (N + BLOCK_N - 1) / BLOCK_N;
+    p.group_m = (tm >= 4 * tn || (precision == 2 && tm * tn > sm_count())) ? 8 / cl : 1;
+    if (gm_env) p.group_m = std::max(1, atoi(gm_env));
+  }
   // AB_GEMM_MN3D=1: an MN-major tile arrives with one 3-D bulk copy instead of one per chunk
   const bool allow_3d = getenv("AB_GEMM_MN3D") != nullptr && getenv("AB_GEMM_NO_MN3D") == nullptr;
   p.a_mn3d = (allow_3d && A.mn_major && M % p.mn_per_chunk == 0 && p.a_chunks > 1) ? 1 : 0;
@@ -611,22 +616,22 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
   p.tiles_n = (N + p.block_n - 1) / p.block_n;
   p.num_tiles = ((M + (long long)cl * BLOCK_M - 1) / ((long long)cl * BLOCK_M)) * p.tiles_n;
   p.num_units = p.num_tiles * p.k_splits;
-  const long long num_tiles = p.num_units;
-  dim3 grid((unsigned)std::min<long long>(num_tiles, sm_count()));  // persistent: one CTA per SM
+  const long long num_units = p.num_units;
+  dim3 grid((unsigned)std::min<long long>(num_units, sm_count()));  // persistent: one CTA per SM
   if (cl > 1) {
     static int resident[2] = {0, 0};  // clusters of this kernel that fit at once (asked once)
     int& res = resident[bf16 ? 1 : 0];
     if (!res) {
       if (bf16) {
-        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-        res = max_clusters(gemm_tc_kernel<1, 4>, cl, smem);
+        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
+        res = max_clusters(gemm_tc_kernel<1, 2>, cl, smem);
       } else {
-        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-        res = max_clusters(gemm_tc_kernel<0, 4>, cl, smem);
+        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
+        res = max_clusters(gemm_tc_kernel<0, 2>, cl, smem);
       }
     }
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(cl * std::min<long long>(num_tiles, res)));
+    cfg.gridDim = dim3((unsigned)(cl * std::min<long long>(num_units, res)));
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
@@ -637,8 +642,8 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    if (bf16) AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<1, 4>, ma[0], ma[1], mb[0], mb[1], p));
-    else AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<0, 4>, ma[0], ma[1], mb[0], mb[1], p));
+    if (bf16) AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<1, 2>, ma[0], ma[1], mb[0], mb[1], p));
+    else AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<0, 2>, ma[0], ma[1], mb[0], mb[1], p));
     g_launches++;
     return splitk_finish(p, st);
   }
@@ -814,4 +819,13 @@ extern "C" int ab_gemm_packed_workspace_bytes(int precision, int64_t m, int64_t 
 
 extern "C" int ab_gemm_tensorcore_eligible(int64_t m, int64_t n, int64_t k) {
   return ab::gemm_tc_eligible(m, n, k) ? 1 : 0;
+}
+
+extern "C" int ab_gemm_max_clusters(int precision, int ctas, int* clusters) {
+  if (!clusters) return ab::fail(AB_ERR_INVALID, "null out pointer");
+  if (ctas < 1 || ctas > 8) return ab::fail(AB_ERR_INVALID, "cluster of %d CTAs", ctas);
+  const void* kern = precision == 2 ? (const void*)ab::gemm_tc_kernel<1, 2> : (const void*)ab::gemm_tc_kernel<0, 2>;
+  AB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ab::kMaxSmemGemm));
+  AB_CUDA(ab::active_clusters(kern, ctas, ab::kMaxSmemGemm, clusters));
+  return AB_OK;
 }

@@ -21,7 +21,7 @@
 // Registers (setmaxnreg, multiples of 8; 512 threads launch with 128 each = 65 536):
 //   producer 24, MMA 160 (d[64] + tot[64] + addressing), epilogue 168:
 //   128 * 24 + 256 * 160 + 128 * 168 = 3 072 + 40 960 + 21 504 = 65 536.
-// The cluster variant's producer, which multicasts, keeps 56 and its (plain) epilogue 136:
+// The CTA pair's producer, which multicasts, keeps 56 and its (plain) epilogue 136:
 //   128 * 56 + 256 * 160 + 128 * 136 = 7 168 + 40 960 + 17 408 = 65 536.
 constexpr int kGemmThreads = kThreads;
 constexpr int kMmaWarp0 = 4;   // first warp of the MMA warpgroups
@@ -969,7 +969,8 @@ __device__ __forceinline__ void mma_kblock(float (&d)[64], uint32_t a_hi, uint32
   }
 }
 
-// CL > 1 (ahead-of-time kernels, AB_GEMM_CLUSTER4): a cluster of CL CTAs stacked along M computes
+// CL > 1 (CL = 2, the CTA pair of the ahead-of-time kernels; see cluster_ctas): a cluster of CL CTAs
+// stacked along M computes
 // one (CL * 128) x 128 tile; they share the B tile, each CTA loading 1/CL of it and multicasting
 // that part into the shared memory of all CL CTAs (cp.async.bulk.tensor ... multicast::cluster).
 // A ring stage of a CTA is then written by every CTA of the cluster, so it is free only when the
@@ -991,12 +992,13 @@ __device__ __forceinline__ void load_b_part(uint8_t* dst, const CUtensorMap* map
   constexpr uint16_t mask = (uint16_t)((1u << CL) - 1u);
   if (!o.mn_major) {
     // K-major: box {128 B of K, block_n / CL rows}, this CTA's rows of the tile
-    tma_load_2d_mc(dst + crank * (b_tile_bytes / CL), map, bar, kc, n0 + (int)crank * (block_n / CL), mask);
+    tma_load_2d_mc_hint(dst + crank * (b_tile_bytes / CL), map, bar, kc, n0 + (int)crank * (block_n / CL), mask,
+                        o.policy);
   } else {
     // MN-major: box {128 B of MN, k_per_kb / CL K rows} per chunk, this CTA's K rows of each chunk
     for (int c = 0; c < o.chunks; ++c)
-      tma_load_2d_mc(dst + c * o.chunk_bytes + crank * (o.chunk_bytes / CL), map, bar, n0 + c * o.mn_per_chunk,
-                     kc + (int)crank * (k_per_kb / CL), mask);
+      tma_load_2d_mc_hint(dst + c * o.chunk_bytes + crank * (o.chunk_bytes / CL), map, bar, n0 + c * o.mn_per_chunk,
+                          kc + (int)crank * (k_per_kb / CL), mask, o.policy);
   }
 }
 

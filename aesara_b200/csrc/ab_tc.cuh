@@ -91,12 +91,12 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
 }
 // the same box delivered to every CTA of `mask` in the cluster, at the same shared-memory offset
 // in each; the complete_tx goes to the barrier at the same offset in each destination CTA
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* map, uint64_t* bar,
-                                               int c0, int c1, uint16_t mask) {
+__device__ __forceinline__ void tma_load_2d_mc_hint(void* smem_dst, const CUtensorMap* map, uint64_t* bar,
+                                                    int c0, int c1, uint16_t mask, uint64_t policy) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      ".L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask), "l"(policy)
       : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -112,7 +112,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
       "r"(cta)
       : "memory");
 }

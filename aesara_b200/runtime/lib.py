@@ -150,6 +150,7 @@ SIGNATURES = {
         C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]
     ),
     "ab_gemm_tensorcore_eligible": (C.c_int, [C.c_int64, C.c_int64, C.c_int64]),
+    "ab_gemm_max_clusters": (C.c_int, [C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "ab_gemm_fused_layout": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "ab_softmax": (
         C.c_int,

@@ -227,6 +227,10 @@ int ab_gemm_packed_fused(int precision, int64_t m, int64_t n, int64_t k, double 
                          const void* Cin, int64_t cin_rs, int64_t cin_cs, void* C, int64_t c_rs,
                          int64_t c_cs, const ab_gemm_epilogue* ep, void* stream);
 int ab_gemm_tensorcore_eligible(int64_t m, int64_t n, int64_t k);
+/* How many clusters of `ctas` CTAs of the ahead-of-time tensor-core GEMM kernel of `precision`
+ * can be resident at once on the current device (cudaOccupancyMaxActiveClusters, full shared
+ * memory): GPCs whose SM count is not a multiple of `ctas` leave SMs idle. */
+int ab_gemm_max_clusters(int precision, int ctas, int* clusters);
 
 /* ---- row ops (SURVEY §8f N1) ---------------------------------------------------
  * The operand is a C-contiguous [outer, r, inner] view; the op runs along r.

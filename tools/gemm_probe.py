@@ -17,17 +17,24 @@ transposed views; bf16 only, TF32 operands are always packed K-major), under the
 Each case is timed in several arms, which take turns window by window so that a drift of the
 clock falls on all of them alike:
 
-    aot       the ahead-of-time kernel with the plain alpha/beta epilogue, as gemm_run picks it;
+    single    the ahead-of-time kernel with the plain alpha/beta epilogue, one CTA per 128 x 128
+              tile (AB_GEMM_CLUSTER=1);
+    pair      the same kernel on CTA pairs stacked along M that share the B tile by TMA
+              multicast (AB_GEMM_CLUSTER=2);
     nvrtc     the fused-epilogue entry point of that layout, built by NVRTC, with the identity
-              region (value 0 = alpha * acc + beta * Cin): the same main loop, the other build;
-    stages4   ``aot`` with a 4-stage operand ring (AB_GEMM_STAGES=4, the fused kernels' ring);
-    group8 / group1   ``aot`` with tile groups of 8 rows / plain row order (AB_GEMM_GROUP_M;
-              square tile grids only).
+              region (value 0 = alpha * acc + beta * Cin), as gemm_run launches it;
+    stages4   ``single`` with a 4-stage operand ring (AB_GEMM_STAGES=4, the fused kernels' ring);
+    group8 / group1   ``single`` with tile groups of 8 rows / plain row order (AB_GEMM_GROUP_M;
+              square tile grids only);
+    pair_group2 / pair_group8   ``pair`` with groups of 2 / 8 pair rows (4 is its default).
 
-Prints one JSON line per case and arm, and a header line with the card, its power limit and
-the NVRTC version; every line carries the SM clock sampled during its timed windows.
+Prints one JSON line per case and arm, and a header line with the card, its power limit, the
+NVRTC version and how many clusters of 2 and of 4 CTAs of the bf16 kernel can be resident at
+once (cudaOccupancyMaxActiveClusters); every line carries the SM clock sampled during its timed
+windows.
 """
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -50,21 +57,25 @@ from bench import ClockSampler  # noqa: E402
 B, H = 65536, 4096
 # name, M, N, K, precision, A layout, B layout -- the layouts of the cfg3 products:
 # X @ W1 (K/K), dW2 = h.T @ dout (both from transposed planes: K/K), dW1 = X.T @ dpre (X read
-# MN-major: MN/K)
+# MN-major: MN/K), dout @ W2.T with W2 read MN-major (K/MN: B not transposed-packed)
 CASES = [
     ("wgrad", H, H, B, 2, "K", "K"),
     ("wgrad", H, H, B, 2, "MN", "K"),
     ("fwd", B, H, H, 2, "K", "K"),
+    ("fwd", B, H, H, 2, "K", "MN"),
     ("fwd", B, H, H, 0, "K", "K"),
     ("wgrad", H, H, B, 0, "K", "K"),
 ]
 POLICY = {0: "fp32", 2: "bf16"}
 ARMS = {  # arm -> (environment, fused)
-    "aot": ({}, False),
+    "single": ({"AB_GEMM_CLUSTER": "1"}, False),
+    "pair": ({"AB_GEMM_CLUSTER": "2"}, False),
     "nvrtc": ({}, True),
-    "stages4": ({"AB_GEMM_STAGES": "4"}, False),
-    "group8": ({"AB_GEMM_GROUP_M": "8"}, False),
-    "group1": ({"AB_GEMM_GROUP_M": "1"}, False),
+    "stages4": ({"AB_GEMM_CLUSTER": "1", "AB_GEMM_STAGES": "4"}, False),
+    "group8": ({"AB_GEMM_CLUSTER": "1", "AB_GEMM_GROUP_M": "8"}, False),
+    "group1": ({"AB_GEMM_CLUSTER": "1", "AB_GEMM_GROUP_M": "1"}, False),
+    "pair_group2": ({"AB_GEMM_CLUSTER": "2", "AB_GEMM_GROUP_M": "2"}, False),
+    "pair_group8": ({"AB_GEMM_CLUSTER": "2", "AB_GEMM_GROUP_M": "8"}, False),
 }
 
 
@@ -200,7 +211,13 @@ def main():
                               "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
     except Exception:
         smi = "unavailable"
-    head = {"device": torch.cuda.get_device_name(0), "nvidia_smi": smi,
+    clusters = {}
+    for ctas in (2, 4):
+        n = ctypes.c_int(0)
+        lib.check(lib.load().ab_gemm_max_clusters(2, ctas, ctypes.byref(n)))
+        clusters[f"max_clusters_{ctas}"] = n.value
+    head = {"device": torch.cuda.get_device_name(0), "nvidia_smi": smi, **clusters,
+            "sms": torch.cuda.get_device_properties(0).multi_processor_count,
             "nvrtc": "%d.%d" % lib.nvrtc_version(), "library": lib.load().ab_version().decode(),
             "window_s": args.window, "repeats": args.repeats}
     print(json.dumps(head), flush=True)
@@ -209,7 +226,7 @@ def main():
         if args.policy != "all" and POLICY[case[4]] != args.policy:
             continue
         tm, tn = -(-case[1] // 128), -(-case[2] // 128)
-        arms = [a for a in want if not (a.startswith("group") and tm >= 4 * tn)]  # square grids only
+        arms = [a for a in want if not ("group" in a and tm >= 4 * tn)]  # square grids only
         for r in run_case(case, arms, max(args.window, 1.0), args.repeats, args.warmup):
             print(json.dumps(r), flush=True)
             rows.append(r)
