@@ -173,27 +173,6 @@ int make_map(CUtensorMap* map, const void* base, bool bf16, long long inner, lon
   return AB_OK;
 }
 
-// MN-major plane [k rows, pitch] as a 3-D tensor {128 B of MN, k, MN chunks}: box = {128 B, box_k
-// rows, chunks} lands as `chunks` consecutive [box_k x 128 B] blocks in shared memory — the
-// canonical MN-major SWIZZLE_128B tile — with one bulk copy.  Needs mn % (128 B of elements) == 0.
-int make_map_mn3d(CUtensorMap* map, const void* base, bool bf16, long long mn, long long k,
-                  long long pitch_elems, int box_k, int chunks) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(AB_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  const int es = bf16 ? 2 : 4;
-  const long long per = SW_BYTES / es;
-  cuuint64_t dims[3] = {(cuuint64_t)per, (cuuint64_t)k, (cuuint64_t)(mn / per)};
-  cuuint64_t strides[2] = {(cuuint64_t)pitch_elems * es, (cuuint64_t)SW_BYTES};
-  cuuint32_t box[3] = {(cuuint32_t)per, (cuuint32_t)box_k, (cuuint32_t)chunks};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
-                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(AB_ERR_CUDA, "cuTensorMapEncodeTiled (3-D) failed with code %d", (int)r);
-  return AB_OK;
-}
-
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 bool eligible(long long M, long long N, long long K) {
@@ -324,25 +303,47 @@ int cluster_ctas(int precision, long long M, bool fused, int k_splits) {
   return (precision == 2 && !fused && M >= 2 * BLOCK_M && k_splits == 1) ? 2 : 1;
 }
 
-template <typename Kern>
-cudaError_t active_clusters(Kern kern, int ctas, size_t smem, int* n) {
+// launch configuration of a persistent grid of `clusters` clusters of `ctas` CTAs; `attr`
+// receives the cluster dimension and has to outlive the use of the result
+cudaLaunchConfig_t cluster_config(int ctas, long long clusters, size_t smem, cudaStream_t st,
+                                  cudaLaunchAttribute* attr) {
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(ctas * (sm_count() / ctas)));
+  cfg.gridDim = dim3((unsigned)(ctas * clusters));
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = ctas;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  cfg.stream = st;
+  attr->id = cudaLaunchAttributeClusterDimension;
+  attr->val.clusterDim.x = ctas;
+  attr->val.clusterDim.y = 1;
+  attr->val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  return cfg;
+}
+
+cudaError_t active_clusters(const void* kern, int ctas, size_t smem, int* n) {
+  cudaLaunchAttribute attr;
+  const cudaLaunchConfig_t cfg = cluster_config(ctas, sm_count() / ctas, smem, nullptr, &attr);
   return cudaOccupancyMaxActiveClusters(n, kern, &cfg);
 }
 
+// the ahead-of-time kernel of (bf16, CTAs per cluster), its dynamic shared memory limit raised
+// on first use
+int plain_kernel(bool bf16, int cl, const void** kern) {
+  static const void* const kernels[2][2] = {
+      {(const void*)gemm_tc_kernel<0, 1>, (const void*)gemm_tc_kernel<0, 2>},
+      {(const void*)gemm_tc_kernel<1, 1>, (const void*)gemm_tc_kernel<1, 2>}};
+  static bool raised[2][2] = {};
+  *kern = kernels[bf16][cl - 1];
+  if (!raised[bf16][cl - 1]) {
+    AB_CUDA(cudaFuncSetAttribute(*kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
+    raised[bf16][cl - 1] = true;
+  }
+  return AB_OK;
+}
+
 // how many clusters of `ctas` CTAs of this kernel can be resident at once (the persistent grid)
-template <typename Kern>
-int max_clusters(Kern kern, int ctas, size_t smem) {
+int max_clusters(const void* kern, int ctas, size_t smem) {
   int n = 0;
   if (active_clusters(kern, ctas, smem, &n) != cudaSuccess || n <= 0) {
     cudaGetLastError();
@@ -449,20 +450,6 @@ int fused_kernel(Module* m, const char* name, cudaKernel_t* out) {
   return AB_OK;
 }
 
-// modules built with AB_EP_STAGED export a marker kernel: their epilogue warps use kStageBytes
-// of shared memory behind the tile accumulator
-bool fused_module_staged(Module* m) {
-  auto it = m->named.find("ab_gemm_ep_staged_marker");
-  if (it != m->named.end()) return it->second != nullptr;
-  cudaKernel_t kern = nullptr;
-  if (cudaLibraryGetKernel(&kern, m->lib, "ab_gemm_ep_staged_marker") != cudaSuccess) {
-    cudaGetLastError();
-    kern = nullptr;
-  }
-  m->named["ab_gemm_ep_staged_marker"] = kern;
-  return kern != nullptr;
-}
-
 int splitk_finish(const GemmParams& p, cudaStream_t st) {
   if (p.k_splits <= 1) return AB_OK;
   const long long work = (p.M * p.N + 3) / 4;
@@ -504,7 +491,7 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
   p.a_kstep = A.mn_major ? mma_k * SW_BYTES : 32;
   p.b_kstep = B.mn_major ? mma_k * SW_BYTES : 32;
   const int stage_bytes = parts * (p.a_tile_bytes + p.b_tile_bytes);
-  const int stage_reserve = kAccBytes + ((ep && fused_module_staged(ep->module)) ? kStageBytes : 0);
+  const int stage_reserve = kAccBytes + (ep ? kStageBytes : 0);  // the fused epilogue's staging chunks
   p.stages = std::max(2, std::min(8, (kMaxSmemGemm - 1024 - stage_reserve) / stage_bytes));
   if (const char* st_env = getenv("AB_GEMM_STAGES"))  // probing knob
     p.stages = std::max(2, std::min(p.stages, atoi(st_env)));
@@ -595,17 +582,11 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     p.group_m = (tm >= 4 * tn || (precision == 2 && tm * tn > sm_count())) ? 8 / cl : 1;
     if (gm_env) p.group_m = std::max(1, atoi(gm_env));
   }
-  // AB_GEMM_MN3D=1: an MN-major tile arrives with one 3-D bulk copy instead of one per chunk
-  const bool allow_3d = getenv("AB_GEMM_MN3D") != nullptr && getenv("AB_GEMM_NO_MN3D") == nullptr;
-  p.a_mn3d = (allow_3d && A.mn_major && M % p.mn_per_chunk == 0 && p.a_chunks > 1) ? 1 : 0;
-  p.b_mn3d = (allow_3d && cl == 1 && B.mn_major && N % p.mn_per_chunk == 0 && p.b_chunks > 1) ? 1 : 0;
   for (int i = 0; i < parts; ++i) {
-    if (p.a_mn3d) rc = make_map_mn3d(&ma[i], A.plane[i], bf16, M, K, A.pitch, p.k_elems_per_row, p.a_chunks);
-    else if (A.mn_major) rc = make_map(&ma[i], A.plane[i], bf16, M, K, A.pitch, p.k_elems_per_row);
+    if (A.mn_major) rc = make_map(&ma[i], A.plane[i], bf16, M, K, A.pitch, p.k_elems_per_row);
     else rc = make_map(&ma[i], A.plane[i], bf16, K, M, A.pitch, BLOCK_M);
     if (rc) return rc;
-    if (p.b_mn3d) rc = make_map_mn3d(&mb[i], B.plane[i], bf16, N, K, B.pitch, p.k_elems_per_row, p.b_chunks);
-    else if (B.mn_major) rc = make_map(&mb[i], B.plane[i], bf16, N, K, B.pitch, p.k_elems_per_row / cl);
+    if (B.mn_major) rc = make_map(&mb[i], B.plane[i], bf16, N, K, B.pitch, p.k_elems_per_row / cl);
     else rc = make_map(&mb[i], B.plane[i], bf16, K, N, B.pitch, p.block_n / cl);
     if (rc) return rc;
   }
@@ -617,36 +598,7 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
   p.num_tiles = ((M + (long long)cl * BLOCK_M - 1) / ((long long)cl * BLOCK_M)) * p.tiles_n;
   p.num_units = p.num_tiles * p.k_splits;
   const long long num_units = p.num_units;
-  dim3 grid((unsigned)std::min<long long>(num_units, sm_count()));  // persistent: one CTA per SM
-  if (cl > 1) {
-    static int resident[2] = {0, 0};  // clusters of this kernel that fit at once (asked once)
-    int& res = resident[bf16 ? 1 : 0];
-    if (!res) {
-      if (bf16) {
-        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-        res = max_clusters(gemm_tc_kernel<1, 2>, cl, smem);
-      } else {
-        AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-        res = max_clusters(gemm_tc_kernel<0, 2>, cl, smem);
-      }
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(cl * std::min<long long>(num_units, res)));
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cl;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (bf16) AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<1, 2>, ma[0], ma[1], mb[0], mb[1], p));
-    else AB_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<0, 2>, ma[0], ma[1], mb[0], mb[1], p));
-    g_launches++;
-    return splitk_finish(p, st);
-  }
+  void* args[] = {&ma[0], &ma[1], &mb[0], &mb[1], &p};
   if (ep) {
     // one entry point per MMA-loop layout (ab_gemm_tc_kernel.cuh, AB_EP_KERNEL)
     static const char* const f16_names[4] = {"ab_gemm_ep_f16", "ab_gemm_ep_f16_km", "ab_gemm_ep_f16_mk",
@@ -654,28 +606,27 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
     const char* name = bf16 ? f16_names[2 * p.a_mn + p.b_mn] : (parts == 2 ? "ab_gemm_ep_tf32" : "ab_gemm_ep_tf32_1p");
     cudaKernel_t kern;
     if ((rc = fused_kernel(ep->module, name, &kern))) return rc;
-    void* args[] = {&ma[0], &ma[1], &mb[0], &mb[1], &p};
+    dim3 grid((unsigned)std::min<long long>(num_units, sm_count()));  // persistent: one CTA per SM
     AB_CUDA(cudaLaunchKernel((const void*)kern, grid, dim3(kThreads), args, smem, st));
     g_launches++;
     return AB_OK;
   }
-  if (bf16) {
-    static bool attr1 = false;
-    if (!attr1) {
-      AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-      attr1 = true;
-    }
-    gemm_tc_kernel<1, 1><<<grid, kThreads, smem, st>>>(ma[0], ma[1], mb[0], mb[1], p);
-  } else {
-    static bool attr0 = false;
-    if (!attr0) {
-      AB_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemGemm));
-      attr0 = true;
-    }
-    gemm_tc_kernel<0, 1><<<grid, kThreads, smem, st>>>(ma[0], ma[1], mb[0], mb[1], p);
-  }
+  const void* kern;
+  if ((rc = plain_kernel(bf16, cl, &kern))) return rc;
+  // persistent: one cluster per SM (cl = 1), or as many pairs as fit at once (asked once per kernel)
+  static int resident[2] = {0, 0};
+  int& res = resident[bf16];
+  if (cl > 1 && !res) res = max_clusters(kern, cl, smem);
+  cudaLaunchAttribute attr;
+  cudaLaunchConfig_t cfg =
+      cluster_config(cl, std::min<long long>(num_units, cl > 1 ? res : sm_count()), smem, st, &attr);
+  // Single CTAs are launched without the attribute: a cluster dimension of 1 is still a cluster
+  // launch, which places the CTAs on the SMs in another order, and the units in flight
+  // (AB_UNIT_DECODE) then share less in L2 (measured on an H100 80GB HBM3, 700 W, at the cfg3
+  // shapes: the bf16 single-CTA kernel ran at 345 instead of 425 TFLOP/s).
+  if (cl == 1) cfg.numAttrs = 0;
+  AB_CUDA(cudaLaunchKernelExC(&cfg, kern, args));
   g_launches++;
-  AB_CUDA(cudaGetLastError());
   return splitk_finish(p, st);
 }
 
@@ -707,25 +658,43 @@ int gemm_tc_f32(int precision, long long M, long long N, long long K, float alph
 }  // namespace ab
 
 // ---- C ABI for callers that keep packed operands across several products -------------
+static int pack_bytes_abi(int precision, int64_t rows, int64_t k, int64_t s_r, int64_t s_k, size_t* bytes,
+                          bool force_k) {
+  if (!bytes) return ab::fail(AB_ERR_INVALID, "null out pointer");
+  *bytes = ab::gemm_pack_bytes(precision, rows, k, s_r, s_k, force_k);
+  return AB_OK;
+}
+
+static ab::PackedOperand from_abi(const ab_gemm_operand& o) {
+  return ab::PackedOperand{{o.plane0, o.plane1}, o.rows, o.k, o.pitch, o.mn_major, o.precision};
+}
+
+static void to_abi(const ab::PackedOperand& po, ab_gemm_operand* out) {
+  out->plane0 = po.plane[0]; out->plane1 = po.plane[1];
+  out->rows = po.rows; out->k = po.k; out->pitch = po.pitch;
+  out->mn_major = po.mn_major; out->precision = po.precision;
+}
+
+static int pack_abi(int precision, const void* src, int64_t rows, int64_t k, int64_t s_r, int64_t s_k,
+                    void* dst, size_t dst_bytes, ab_gemm_operand* out, void* stream, bool force_k) {
+  if (!out) return ab::fail(AB_ERR_INVALID, "null ab_gemm_operand");
+  ab::PackedOperand po{};
+  int rc = ab::gemm_pack(precision, static_cast<const float*>(src), rows, k, s_r, s_k, dst,
+                         dst_bytes, &po, ab::as_stream(stream), force_k);
+  if (rc) return rc;
+  to_abi(po, out);
+  return AB_OK;
+}
+
 extern "C" int ab_gemm_pack_bytes(int precision, int64_t rows, int64_t k, int64_t s_r, int64_t s_k,
                                   size_t* bytes) {
-  if (!bytes) return ab::fail(AB_ERR_INVALID, "null out pointer");
-  *bytes = ab::gemm_pack_bytes(precision, rows, k, s_r, s_k);
-  return AB_OK;
+  return pack_bytes_abi(precision, rows, k, s_r, s_k, bytes, false);
 }
 
 extern "C" int ab_gemm_pack(int precision, const void* src, int64_t rows, int64_t k, int64_t s_r,
                             int64_t s_k, void* dst, size_t dst_bytes, ab_gemm_operand* out,
                             void* stream) {
-  if (!out) return ab::fail(AB_ERR_INVALID, "null ab_gemm_operand");
-  ab::PackedOperand po{};
-  int rc = ab::gemm_pack(precision, static_cast<const float*>(src), rows, k, s_r, s_k, dst,
-                         dst_bytes, &po, ab::as_stream(stream));
-  if (rc) return rc;
-  out->plane0 = po.plane[0]; out->plane1 = po.plane[1];
-  out->rows = po.rows; out->k = po.k; out->pitch = po.pitch;
-  out->mn_major = po.mn_major; out->precision = po.precision;
-  return AB_OK;
+  return pack_abi(precision, src, rows, k, s_r, s_k, dst, dst_bytes, out, stream, false);
 }
 
 // The same with the planes forced K-major ([rows, pitch], K contiguous) whatever the strides:
@@ -735,23 +704,13 @@ extern "C" int ab_gemm_pack(int precision, const void* src, int64_t rows, int64_
 // only be read K-major.
 extern "C" int ab_gemm_pack_kmajor_bytes(int precision, int64_t rows, int64_t k, int64_t s_r,
                                          int64_t s_k, size_t* bytes) {
-  if (!bytes) return ab::fail(AB_ERR_INVALID, "null out pointer");
-  *bytes = ab::gemm_pack_bytes(precision, rows, k, s_r, s_k, true);
-  return AB_OK;
+  return pack_bytes_abi(precision, rows, k, s_r, s_k, bytes, true);
 }
 
 extern "C" int ab_gemm_pack_kmajor(int precision, const void* src, int64_t rows, int64_t k,
                                    int64_t s_r, int64_t s_k, void* dst, size_t dst_bytes,
                                    ab_gemm_operand* out, void* stream) {
-  if (!out) return ab::fail(AB_ERR_INVALID, "null ab_gemm_operand");
-  ab::PackedOperand po{};
-  int rc = ab::gemm_pack(precision, static_cast<const float*>(src), rows, k, s_r, s_k, dst,
-                         dst_bytes, &po, ab::as_stream(stream), true);
-  if (rc) return rc;
-  out->plane0 = po.plane[0]; out->plane1 = po.plane[1];
-  out->rows = po.rows; out->k = po.k; out->pitch = po.pitch;
-  out->mn_major = po.mn_major; out->precision = po.precision;
-  return AB_OK;
+  return pack_abi(precision, src, rows, k, s_r, s_k, dst, dst_bytes, out, stream, true);
 }
 
 extern "C" int ab_gemm_packed(int precision, int64_t m, int64_t n, int64_t k, double alpha,
@@ -762,8 +721,7 @@ extern "C" int ab_gemm_packed(int precision, int64_t m, int64_t n, int64_t k, do
   if (!A || !B) return ab::fail(AB_ERR_INVALID, "null packed operand");
   if (!ab::gemm_tc_eligible(m, n, k))
     return ab::fail(AB_ERR_UNSUPPORTED, "problem too small for the tensor-core path; use ab_gemm");
-  ab::PackedOperand pa{{A->plane0, A->plane1}, A->rows, A->k, A->pitch, A->mn_major, A->precision};
-  ab::PackedOperand pb{{B->plane0, B->plane1}, B->rows, B->k, B->pitch, B->mn_major, B->precision};
+  const ab::PackedOperand pa = from_abi(*A), pb = from_abi(*B);
   return ab::gemm_run(precision, m, n, k, (float)alpha, pa, pb, (float)beta, static_cast<float*>(C),
                       c_rs, c_cs, ab::as_stream(stream), static_cast<const float*>(Cin), cin_rs,
                       cin_cs, workspace, workspace_bytes);
@@ -777,8 +735,7 @@ extern "C" int ab_gemm_packed_fused(int precision, int64_t m, int64_t n, int64_t
   if (!A || !B || !ep || !ep->module) return ab::fail(AB_ERR_INVALID, "null argument");
   if (!ab::gemm_tc_eligible(m, n, k))
     return ab::fail(AB_ERR_UNSUPPORTED, "problem too small for the tensor-core path");
-  ab::PackedOperand pa{{A->plane0, A->plane1}, A->rows, A->k, A->pitch, A->mn_major, A->precision};
-  ab::PackedOperand pb{{B->plane0, B->plane1}, B->rows, B->k, B->pitch, B->mn_major, B->precision};
+  const ab::PackedOperand pa = from_abi(*A), pb = from_abi(*B);
   ab::EpilogueSpec spec;
   spec.module = reinterpret_cast<ab::Module*>(ep->module);
   spec.nops = ep->n_operands;
@@ -824,8 +781,8 @@ extern "C" int ab_gemm_tensorcore_eligible(int64_t m, int64_t n, int64_t k) {
 extern "C" int ab_gemm_max_clusters(int precision, int ctas, int* clusters) {
   if (!clusters) return ab::fail(AB_ERR_INVALID, "null out pointer");
   if (ctas < 1 || ctas > 8) return ab::fail(AB_ERR_INVALID, "cluster of %d CTAs", ctas);
-  const void* kern = precision == 2 ? (const void*)ab::gemm_tc_kernel<1, 2> : (const void*)ab::gemm_tc_kernel<0, 2>;
-  AB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ab::kMaxSmemGemm));
+  const void* kern;
+  if (int rc = ab::plain_kernel(precision == 2, 2, &kern)) return rc;
   AB_CUDA(ab::active_clusters(kern, ctas, ab::kMaxSmemGemm, clusters));
   return AB_OK;
 }

@@ -57,8 +57,6 @@ struct GemmParams {
   int k_elems_per_row;    // K elements per stage = per 128-byte K-major row: 32 (tf32) / 64 (bf16)
   int a_tile_bytes, b_tile_bytes;
   int a_mn, b_mn;         // operand is MN-major
-  int a_mn3d, b_mn3d;     // ... and its tensor map is 3-D {128 B of MN, K rows, MN chunks}: the
-                          // whole tile arrives with ONE bulk copy instead of one per chunk
   int a_chunks, b_chunks; // MN-major: 128-byte MN chunks per tile (tile_rows * elem_size / 128)
   int chunk_bytes;        // MN-major: k_elems_per_row rows * 128 B
   int mn_per_chunk;       // MN-major: elements per chunk (128 / elem_size)
@@ -110,21 +108,19 @@ struct GemmParams {
 // a field read through `p` inside the loop is re-loaded (LDCU + dependent UISETP) after each
 // of them, on the single producer thread's critical path.
 struct OperandLoad {
-  int mn_major, chunks, mn3d, chunk_bytes, mn_per_chunk;
+  int mn_major, chunks, chunk_bytes, mn_per_chunk;
   uint64_t policy;
 };
 __device__ __forceinline__ OperandLoad operand_load_a(const GemmParams& p) {
-  return OperandLoad{p.a_mn, p.a_chunks, p.a_mn3d, p.chunk_bytes, p.mn_per_chunk, make_l2_policy(p.a_l2)};
+  return OperandLoad{p.a_mn, p.a_chunks, p.chunk_bytes, p.mn_per_chunk, make_l2_policy(p.a_l2)};
 }
 __device__ __forceinline__ OperandLoad operand_load_b(const GemmParams& p) {
-  return OperandLoad{p.b_mn, p.b_chunks, p.b_mn3d, p.chunk_bytes, p.mn_per_chunk, make_l2_policy(p.b_l2)};
+  return OperandLoad{p.b_mn, p.b_chunks, p.chunk_bytes, p.mn_per_chunk, make_l2_policy(p.b_l2)};
 }
 __device__ __forceinline__ void load_tile(uint8_t* dst, const CUtensorMap* map, uint64_t* bar,
                                           int kc, int mn0, const OperandLoad& o) {
   if (!o.mn_major) {
     tma_load_2d_hint(dst, map, bar, kc, mn0, o.policy);
-  } else if (o.mn3d) {
-    tma_load_3d(dst, map, bar, 0, kc, mn0 / o.mn_per_chunk);
   } else {
     for (int c = 0; c < o.chunks; ++c)
       tma_load_2d_hint(dst + c * o.chunk_bytes, map, bar, mn0 + c * o.mn_per_chunk, kc, o.policy);
@@ -193,72 +189,38 @@ __device__ __forceinline__ void acc_ld_x32(uint32_t acc_base, int r, int c0, flo
 // C[row, n0 + ...] = alpha * acc + beta * Cin for one thread's row and column range
 // 8 consecutive floats as two 128-bit accesses (16-byte alignment is the caller's precondition;
 // sm_90 has no 256-bit global access)
-#define AB_HAS_V8 0
 // STREAM: the access belongs to a fused epilogue region -- [M, N] operands read once and values
 // written once, far larger than L2: evict-first, so that they do not push the products' small
 // operand (a weight matrix, GemmParams::b_l2) out of L2.  The plain alpha/beta epilogue keeps
 // the default policy (a small result is usually the next node's operand).
 template <bool STREAM>
-__device__ __forceinline__ void ld8(const float* q, float (&o)[8], bool wide) {
-#if AB_HAS_V8
-  if (wide) {
-    if (STREAM)
-      asm volatile("ld.global.L1::no_allocate.L2::evict_first.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                   : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]), "=f"(o[4]), "=f"(o[5]), "=f"(o[6]), "=f"(o[7])
-                   : "l"(q));
-    else
-      asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                   : "=f"(o[0]), "=f"(o[1]), "=f"(o[2]), "=f"(o[3]), "=f"(o[4]), "=f"(o[5]), "=f"(o[6]), "=f"(o[7])
-                   : "l"(q));
-  } else
-#endif
-  {
-    const float4 a = STREAM ? __ldcs(reinterpret_cast<const float4*>(q)) : *reinterpret_cast<const float4*>(q);
-    const float4 b = STREAM ? __ldcs(reinterpret_cast<const float4*>(q + 4)) : *reinterpret_cast<const float4*>(q + 4);
-    o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; o[4] = b.x; o[5] = b.y; o[6] = b.z; o[7] = b.w;
-  }
+__device__ __forceinline__ void ld8(const float* q, float (&o)[8]) {
+  const float4 a = STREAM ? __ldcs(reinterpret_cast<const float4*>(q)) : *reinterpret_cast<const float4*>(q);
+  const float4 b = STREAM ? __ldcs(reinterpret_cast<const float4*>(q + 4)) : *reinterpret_cast<const float4*>(q + 4);
+  o[0] = a.x; o[1] = a.y; o[2] = a.z; o[3] = a.w; o[4] = b.x; o[5] = b.y; o[6] = b.z; o[7] = b.w;
 }
 template <bool STREAM>
-__device__ __forceinline__ void st8(float* q, const float (&v)[8], bool wide) {
-#if AB_HAS_V8
-  if (wide) {
-    if (STREAM)
-      asm volatile("st.global.L2::evict_first.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(q), "f"(v[0]), "f"(v[1]),
-                   "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-                   : "memory");
-    else
-      asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(q), "f"(v[0]), "f"(v[1]), "f"(v[2]),
-                   "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-                   : "memory");
-  } else
-#endif
-  {
-    if (STREAM) {
-      __stcs(reinterpret_cast<float4*>(q), make_float4(v[0], v[1], v[2], v[3]));
-      __stcs(reinterpret_cast<float4*>(q + 4), make_float4(v[4], v[5], v[6], v[7]));
-    } else {
-      *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
-      *reinterpret_cast<float4*>(q + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    }
+__device__ __forceinline__ void st8(float* q, const float (&v)[8]) {
+  if (STREAM) {
+    __stcs(reinterpret_cast<float4*>(q), make_float4(v[0], v[1], v[2], v[3]));
+    __stcs(reinterpret_cast<float4*>(q + 4), make_float4(v[4], v[5], v[6], v[7]));
+  } else {
+    *reinterpret_cast<float4*>(q) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(q + 4) = make_float4(v[4], v[5], v[6], v[7]);
   }
 }
 
-#ifndef AB_EP_STAGED
-#define AB_EP_STAGED 0
-#endif
 constexpr int kStageBytesPerWarp = 32 * 32 * 4;                     // one 32 x 32 float32 chunk
 constexpr int kStageBytes = (kEpiThreads / 32) * kStageBytesPerWarp;  // behind the operand ring
 
 struct EpilogueOut {
   const GemmParams& p;
-  bool vec_ok, wide_out, wide_in;
-  uint32_t stage;  // AB_EP_STAGED builds: shared-space address of this warp's 4 KB (see fused_reduce)
+  bool vec_ok;
+  uint32_t stage;  // fused regions: shared-space address of this warp's 4 KB (see fused_reduce)
   __device__ explicit EpilogueOut(const GemmParams& p_, uint32_t stage_ = 0) : p(p_), stage(stage_) {
     vec_ok = (p.c_cs == 1) && ((p.c_rs & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) &&
              (p.beta == 0.0f || ((p.cin_cs == 1) && ((p.cin_rs & 3) == 0) &&
                                  ((reinterpret_cast<uintptr_t>(p.Cin) & 15) == 0)));
-    wide_out = ((p.c_rs & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 31) == 0);
-    wide_in = ((p.cin_rs & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.Cin) & 31) == 0);
   }
   // split-K: alpha * acc of K range `split` (>= 1) into its [M, N] scratch plane
   __device__ __forceinline__ void store_partial(const float (&acc)[kAccRegs], long long row,
@@ -294,8 +256,6 @@ struct EpilogueOut {
       if (c < nchunks) {
         const long long col0 = n0 + c * 32;
         if (vec_ok && col0 + 32 <= p.N) {
-          // 8 columns per step: one 256-bit access per 32-byte sector where the rows are
-          // 32-byte aligned (each L2 sector is touched by one request instead of two)
 #pragma unroll
           for (int j = 0; j < 32; j += 8) {
             float v[8];
@@ -303,11 +263,11 @@ struct EpilogueOut {
             for (int t = 0; t < 8; ++t) v[t] = p.alpha * acc[c * 32 + j + t];
             if (p.beta != 0.0f) {
               float o[8];
-              ld8<false>(irow + col0 + j, o, wide_in);
+              ld8<false>(irow + col0 + j, o);
 #pragma unroll
               for (int t = 0; t < 8; ++t) v[t] += p.beta * o[t];
             }
-            st8<false>(crow + col0 + j, v, wide_out);
+            st8<false>(crow + col0 + j, v);
           }
         } else {
 #pragma unroll
@@ -369,16 +329,15 @@ struct EpilogueOut {
     }
     return s;
   }
-  // SKIP: the value that leaves through the shared-memory staging buffer instead (-1: none)
-  template <int SKIP>
+  // every value but kStageValue, which leaves through the shared-memory staging buffer instead
   __device__ __forceinline__ void put_outputs(const float (&o)[AB_EP_NOUT][8], long long row, long long col) const {
 #pragma unroll
     for (int k = 0; k < AB_EP_NOUT; ++k) {
-      if (k == SKIP) continue;
+      if (k == kStageValue) continue;
       float* dst = k == 0 ? p.C : p.out_ptr[k];
       const long long rs = k == 0 ? p.c_rs : p.out_rs[k];
       if (dst)
-        st8<true>(dst + row * rs + col, o[k], ((rs & 7) == 0) && ((reinterpret_cast<uintptr_t>(dst) & 31) == 0));
+        st8<true>(dst + row * rs + col, o[k]);
       if (p.shadow[k]) {
         uint32_t h[4];
 #pragma unroll
@@ -412,84 +371,51 @@ struct EpilogueOut {
 #endif
   static __device__ __forceinline__ constexpr bool is_row_op(int k) { return ((AB_EP_ROWMASK >> k) & 1) != 0; }
   struct ChunkPre {
-    // [M, N] reads of the next chunk.  Register-only builds: this lane's row, 32 columns.
-    // AB_EP_STAGED builds: the COALESCED layout -- q[i] = row 4 i + lane / 8 of the warp's 32,
-    // columns 4 (lane % 8) .. + 3, so that every LDG.128 covers four full 128-byte lines
-    // (read row-per-lane, an instruction touches 32 lines, 16 bytes of each: the loads then
-    // queue in the LSU) -- and turned
-    // into the row-per-lane layout through the staging buffer at the top of fused_eval.
+    // [M, N] reads of the next chunk in the COALESCED layout -- q[i] = row 4 i + lane / 8 of the
+    // warp's 32, columns 4 (lane % 8) .. + 3, so that every LDG.128 covers four full 128-byte
+    // lines (read row-per-lane, an instruction touches 32 lines, 16 bytes of each: the loads
+    // then queue in the LSU) -- and turned into the row-per-lane layout through the staging
+    // buffer at the top of fused_eval.
 #if AB_EP_CIN
-#if AB_EP_STAGED
     float4 cinq[8];
-#else
-    float cin[32];
-#endif
 #endif
 #if AB_EP_PRE_OP >= 0
-#if AB_EP_STAGED
     float4 opq[8];
-#else
-    float op[32];
-#endif
 #endif
     float vec[AB_EP_NOPS > 0 ? AB_EP_NOPS : 1];
   };
-  __device__ __forceinline__ void prefetch_chunk(ChunkPre& pre, long long row, long long col0, bool live,
+  __device__ __forceinline__ void prefetch_chunk(ChunkPre& pre, long long row, long long col0,
                                                  const FusedScalars& sc, int lane) const {
-    const long long r = live ? row : 0;
-    (void)r; (void)sc; (void)pre; (void)col0;
 #pragma unroll
     for (int k = 0; k < AB_EP_NOPS; ++k) {
       if (sc.vec[k] && !is_row_op(k)) {
         pre.vec[k] = (col0 + lane < p.N) ? __ldg(p.ep_ptr[k] + col0 + lane) : 0.0f;
       }
     }
-#if AB_EP_STAGED
-    {
-      const long long row0 = row - lane, col = col0 + 4 * (lane & 7);
-      (void)row0; (void)col;
+    const long long row0 = row - lane, col = col0 + 4 * (lane & 7);
+    (void)row0; (void)col;
 #if AB_EP_CIN
-      if (p.beta != 0.0f) {
+    if (p.beta != 0.0f) {
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const long long grow = row0 + 4 * i + (lane >> 3);
-          pre.cinq[i] = (grow < p.M && col < p.N) ? __ldcs(reinterpret_cast<const float4*>(p.Cin + grow * p.cin_rs + col))
-                                                  : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        }
+      for (int i = 0; i < 8; ++i) {
+        const long long grow = row0 + 4 * i + (lane >> 3);
+        pre.cinq[i] = (grow < p.M && col < p.N) ? __ldcs(reinterpret_cast<const float4*>(p.Cin + grow * p.cin_rs + col))
+                                                : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
       }
-#endif
-#if AB_EP_PRE_OP >= 0
-      if (!sc.is[AB_EP_PRE_OP] && p.ep_cs[AB_EP_PRE_OP] == 1) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const long long grow = row0 + 4 * i + (lane >> 3);
-          pre.opq[i] = (grow < p.M && col < p.N)
-                           ? __ldcs(reinterpret_cast<const float4*>(p.ep_ptr[AB_EP_PRE_OP] + grow * p.ep_rs[AB_EP_PRE_OP] + col))
-                           : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        }
-      }
-#endif
-    }
-#else
-#if AB_EP_CIN
-    if (live && p.beta != 0.0f) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 8)
-        if (col0 + j < p.N) ld8<true>(p.Cin + r * p.cin_rs + col0 + j, *reinterpret_cast<float(*)[8]>(&pre.cin[j]), wide_in);
     }
 #endif
 #if AB_EP_PRE_OP >= 0
-    if (live && !sc.is[AB_EP_PRE_OP] && p.ep_cs[AB_EP_PRE_OP] == 1) {
-      const bool wide = ((reinterpret_cast<uintptr_t>(p.ep_ptr[AB_EP_PRE_OP]) & 31) == 0) && ((p.ep_rs[AB_EP_PRE_OP] & 7) == 0);
+    if (!sc.is[AB_EP_PRE_OP] && p.ep_cs[AB_EP_PRE_OP] == 1) {
 #pragma unroll
-      for (int j = 0; j < 32; j += 8)
-        if (col0 + j < p.N)
-          ld8<true>(p.ep_ptr[AB_EP_PRE_OP] + r * p.ep_rs[AB_EP_PRE_OP] + col0 + j, *reinterpret_cast<float(*)[8]>(&pre.op[j]), wide);
+      for (int i = 0; i < 8; ++i) {
+        const long long grow = row0 + 4 * i + (lane >> 3);
+        pre.opq[i] = (grow < p.M && col < p.N)
+                         ? __ldcs(reinterpret_cast<const float4*>(p.ep_ptr[AB_EP_PRE_OP] + grow * p.ep_rs[AB_EP_PRE_OP] + col))
+                         : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      }
     }
-#endif
 #endif
   }
-#if AB_EP_STAGED
   // coalesced layout (ChunkPre) -> this lane's row, through the staging buffer
   __device__ __forceinline__ void restage(const float4 (&q)[8], float (&out)[32], int lane) const {
 #pragma unroll
@@ -502,26 +428,24 @@ struct EpilogueOut {
     }
     __syncwarp();
   }
-#endif
   // ---- one 32-column chunk of one accumulator row, in two parts -------------------------
   // fused_eval:   x[32] (raw accumulator values of columns col0 .. col0+31 of `row`) -> the
   //               region's values; consumes the read-ahead buffer `pre`, stores the outputs and
   //               their natural bf16 planes, adds to the thread's total `fs`, and leaves the
-  //               value that is reduced / transposed in x[] (0 for rows and columns outside).
-  // fused_reduce: the cross-lane part: column sums of the warp's 32 rows and the transposed
-  //               bf16 plane.
+  //               value that is reduced / transposed in the staging buffer (0 for rows and
+  //               columns outside).
+  // fused_reduce: the cross-lane part, from the staging buffer: the coalesced store of that
+  //               value, column sums of the warp's 32 rows and the transposed bf16 plane.
   // The caller issues the NEXT chunk's reads between the two: `pre` is dead after fused_eval,
-  // and the ~300 shuffle/select instructions of fused_reduce give those reads their latency.
+  // and the shared-memory passes of fused_reduce give those reads their latency.
   // (Two alternating buffers and a loop body of two chunks would do the same at twice the code,
   // and the larger body waits on instruction fetch.)
-  __device__ __forceinline__ void fused_eval(float (&x)[32], long long row, long long col0, bool live,
+  __device__ __forceinline__ void fused_eval(const float (&x)[32], long long row, long long col0, bool live,
                                              int lane, const FusedScalars& sc, FF& fs, const ChunkPre& pre) const {
     const long long r = live ? row : 0;
-    (void)lane; (void)fs;
 #if AB_EP_PRE_OP >= 0
     const bool pre_ok = live && !sc.is[AB_EP_PRE_OP] && p.ep_cs[AB_EP_PRE_OP] == 1;
 #endif
-#if AB_EP_STAGED
 #if AB_EP_CIN
     float cin_l[32];
     if (p.beta != 0.0f) restage(pre.cinq, cin_l, lane);
@@ -529,14 +453,6 @@ struct EpilogueOut {
 #if AB_EP_PRE_OP >= 0
     float op_l[32];
     if (!sc.is[AB_EP_PRE_OP] && p.ep_cs[AB_EP_PRE_OP] == 1) restage(pre.opq, op_l, lane);
-#endif
-#else
-#if AB_EP_CIN
-    const float (&cin_l)[32] = pre.cin;
-#endif
-#if AB_EP_PRE_OP >= 0
-    const float (&op_l)[32] = pre.op;
-#endif
 #endif
 #pragma unroll
     for (int j = 0; j < 32; j += 8) {
@@ -567,7 +483,7 @@ struct EpilogueOut {
           for (int t = 0; t < 8; ++t) v[t] += p.beta * cin_l[j + t];
 #else
           float ci[8];
-          ld8<true>(p.Cin + r * p.cin_rs + col, ci, wide_in);
+          ld8<true>(p.Cin + r * p.cin_rs + col, ci);
 #pragma unroll
           for (int t = 0; t < 8; ++t) v[t] += p.beta * ci[t];
 #endif
@@ -589,8 +505,7 @@ struct EpilogueOut {
 #pragma unroll
             for (int t = 0; t < 8; ++t) e[k][t] = sc.v[k];
           } else if (p.ep_cs[k] == 1) {
-            ld8<true>(p.ep_ptr[k] + r * p.ep_rs[k] + col, e[k],
-                ((reinterpret_cast<uintptr_t>(p.ep_ptr[k]) & 31) == 0) && ((p.ep_rs[k] & 7) == 0));
+            ld8<true>(p.ep_ptr[k] + r * p.ep_rs[k] + col, e[k]);
           } else {
             const float* q = p.ep_ptr[k] + r * p.ep_rs[k] + col * p.ep_cs[k];
 #pragma unroll
@@ -600,20 +515,9 @@ struct EpilogueOut {
         float o[AB_EP_NOUT][8];
 #pragma unroll
         for (int t = 0; t < 8; ++t) { AB_EP_EVAL(v[t], e, t, o); }
-#if AB_EP_STAGED
-        put_outputs<kStageValue>(o, r, col);
+        put_outputs(o, r, col);
         sts128(stage + 4u * st_off(lane, j >> 2), o[kStageValue][0], o[kStageValue][1], o[kStageValue][2], o[kStageValue][3]);
         sts128(stage + 4u * st_off(lane, (j >> 2) + 1), o[kStageValue][4], o[kStageValue][5], o[kStageValue][6], o[kStageValue][7]);
-#else
-        put_outputs<-1>(o, r, col);
-#if AB_EP_COLSUM >= 0
-#pragma unroll
-        for (int t = 0; t < 8; ++t) x[j + t] = o[AB_EP_COLSUM][t];
-#elif AB_EP_TPLANE >= 0
-#pragma unroll
-        for (int t = 0; t < 8; ++t) x[j + t] = o[AB_EP_TPLANE][t];
-#endif
-#endif
 #if AB_EP_FULLSUM >= 0
 #if AB_EP_EXACT_SUMS
         {
@@ -642,17 +546,12 @@ struct EpilogueOut {
 #endif
 #endif
       } else {
-#if AB_EP_STAGED
         sts128(stage + 4u * st_off(lane, j >> 2), 0.0f, 0.0f, 0.0f, 0.0f);
         sts128(stage + 4u * st_off(lane, (j >> 2) + 1), 0.0f, 0.0f, 0.0f, 0.0f);
-#elif AB_EP_COLSUM >= 0 || AB_EP_TPLANE >= 0
-#pragma unroll
-        for (int t = 0; t < 8; ++t) x[j + t] = 0.0f;
-#endif
       }
     }
   }
-  // ---- AB_EP_STAGED: the value that is stored / reduced / transposed goes through 4 KB of
+  // ---- The value that is stored / reduced / transposed goes through 4 KB of
   // shared memory per warp (a 32 x 32 float32 chunk, 16-byte groups XOR-swizzled with the row:
   // the SWIZZLE_128B pattern, conflict-free for the row writes of fused_eval, for the row
   // reads of pass 1 and for the column reads of pass 2):
@@ -660,15 +559,13 @@ struct EpilogueOut {
   //           line (float32 output) / 64 contiguous bytes (bf16 plane).  Stored from the
   //           accumulator layout (lane = row) every STG touches 32 different lines, half a
   //           sector each, and the epilogue warps wait on the store queue;
-  //   pass 2  lane c reads column c (32 LDS, one per row): the transpose that took 48 shuffles
-  //           and ~130 selects, and the column sum becomes 31 adds without any shuffle.
+  //   pass 2  lane c reads column c (32 LDS, one per row): the transpose needs no shuffle, and
+  //           the column sum is 31 adds.
   // The buffers (4 warps x 4 KB) live behind the tile's accumulator, at the end of the operand
-  // ring: the bf16 / tf32 ring keeps 4 stages with them (5 without), the hi/lo ring 2.
+  // ring: the bf16 / tf32 ring keeps 4 stages with them, the hi/lo ring 2.
   static constexpr int kStageValue = AB_EP_COLSUM >= 0 ? AB_EP_COLSUM : (AB_EP_TPLANE >= 0 ? AB_EP_TPLANE : 0);
   static __device__ __forceinline__ uint32_t st_off(int r, int g) { return (uint32_t)(r * 32 + ((g ^ (r & 7)) << 2)); }
-#if AB_EP_STAGED
-  __device__ __forceinline__ void fused_reduce(float (&x)[32], long long row, long long col0, int lane) const {
-    (void)x;
+  __device__ __forceinline__ void fused_reduce(long long row, long long col0, int lane) const {
     __syncwarp();
     const long long row0 = row - lane;
     {
@@ -773,121 +670,6 @@ struct EpilogueOut {
 #endif
     __syncwarp();  // the buffer is free for the next chunk's values
   }
-#else
-  __device__ __forceinline__ void fused_reduce(float (&x)[32], long long row, long long col0, int lane) const {
-    (void)x; (void)row; (void)col0; (void)lane;
-#if AB_EP_TPLANE >= 0
-    // Transposed bf16 plane, first half: rows are lanes, so two vertically adjacent values sit
-    // in lanes l and l ^ 1.  Even lanes keep the even columns, odd lanes the odd ones: after
-    // one exchange, P[i] of lane l is column 2 i + (l & 1) of the row pair (l & ~1, l | 1),
-    // packed (low half = even row).  The remaining four exchanges (below, after the column
-    // sums have consumed x[]) work on 16 packed registers instead of 32 floats.
-    uint32_t P[16];
-    const bool want_t = p.shadow_t != nullptr;
-    if (want_t) {
-      const bool odd = (lane & 1) != 0;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const float mine = odd ? x[2 * i + 1] : x[2 * i];
-        const float send = odd ? x[2 * i] : x[2 * i + 1];
-        const float got = __shfl_xor_sync(0xffffffffu, send, 1);
-        uint32_t h;  // low half <- second source operand
-        asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(got), "f"(mine));
-        P[i] = __byte_perm(h, 0u, odd ? 0x1032u : 0x3210u);
-      }
-    }
-#endif
-#if AB_EP_COLSUM >= 0
-    {
-      // 32 x 32 transpose-reduce over the warp's rows: after the step with distance h every
-      // lane keeps the half of its columns selected by bit h of its lane index; lane l ends
-      // with the sum of column col0 + l.  The reference's CAReduce accumulates float32 sums in
-      // float64 (tensor/elemwise.py:1371-1385): under the fp32-faithful policy the 32 rows are
-      // added as float pairs (see FF above); under the tf32 / bf16 policies -- the addends
-      // carry 2^-11 / 2^-8 relative error themselves -- as a float32 tree.  Either way the
-      // partial sum leaves the warp as float64.
-      const long long rb = row >> 5;  // row - lane is a multiple of 32
-#if AB_EP_EXACT_SUMS
-      FF d[16];
-      {
-        const bool up = (lane & 16) != 0;
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float keep = up ? x[16 + i] : x[i];
-          const float send = up ? x[i] : x[16 + i];
-          d[i].hi = keep;
-          d[i].lo = 0.0f;
-          ff_add(d[i], __shfl_xor_sync(0xffffffffu, send, 16));
-        }
-      }
-#define AB_COLSUM_STEP(H)                                                      \
-      {                                                                        \
-        const bool up = (lane & (H)) != 0;                                     \
-        _Pragma("unroll") for (int i = 0; i < (H); ++i) {                      \
-          const FF keep = up ? d[(H) + i] : d[i];                              \
-          const FF send = up ? d[i] : d[(H) + i];                              \
-          FF got;                                                              \
-          got.hi = __shfl_xor_sync(0xffffffffu, send.hi, (H));                 \
-          got.lo = __shfl_xor_sync(0xffffffffu, send.lo, (H));                 \
-          d[i] = keep;                                                         \
-          ff_add(d[i], got);                                                   \
-        }                                                                      \
-      }
-      AB_COLSUM_STEP(8) AB_COLSUM_STEP(4) AB_COLSUM_STEP(2) AB_COLSUM_STEP(1)
-#undef AB_COLSUM_STEP
-      if (rb * 32 < p.M && col0 + lane < p.N) p.colsum_ws[rb * p.N + col0 + lane] = ff_double(d[0]);
-#else
-#define AB_COLSUM_STEP(H)                                                      \
-      {                                                                        \
-        const bool up = (lane & (H)) != 0;                                     \
-        _Pragma("unroll") for (int i = 0; i < (H); ++i) {                      \
-          const float keep = up ? x[(H) + i] : x[i];                           \
-          const float send = up ? x[i] : x[(H) + i];                           \
-          x[i] = __fadd_rn(keep, __shfl_xor_sync(0xffffffffu, send, (H)));     \
-        }                                                                      \
-      }
-      AB_COLSUM_STEP(16) AB_COLSUM_STEP(8) AB_COLSUM_STEP(4) AB_COLSUM_STEP(2) AB_COLSUM_STEP(1)
-#undef AB_COLSUM_STEP
-      if (rb * 32 < p.M && col0 + lane < p.N) p.colsum_ws[rb * p.N + col0 + lane] = (double)x[0];
-#endif
-    }
-#endif
-#if AB_EP_TPLANE >= 0
-    if (want_t) {
-      // second half: register index bit b <-> lane bit b + 1 (b = 0..3).  Before: lane bits
-      // 1..4 = row pair k, register index i = column / 2.  After: lane l = column col0 + l,
-      // P[k] = rows (row0 + 2 k, row0 + 2 k + 1): 64 contiguous bytes of the transposed plane.
-#define AB_T_STEP(B)                                                            \
-      {                                                                         \
-        const bool up = (lane & (2 << (B))) != 0;                               \
-        _Pragma("unroll") for (int i = 0; i < 16; ++i) {                        \
-          if ((i & (1 << (B))) == 0) {                                          \
-            const uint32_t send = up ? P[i] : P[i | (1 << (B))];                \
-            const uint32_t got = __shfl_xor_sync(0xffffffffu, send, 2 << (B));  \
-            if (up) P[i] = got; else P[i | (1 << (B))] = got;                   \
-          }                                                                     \
-        }                                                                       \
-      }
-      AB_T_STEP(0) AB_T_STEP(1) AB_T_STEP(2) AB_T_STEP(3)
-#undef AB_T_STEP
-      const long long row0 = row - lane;
-      const long long c = col0 + lane;
-      if (c < p.N && row0 < p.M) {
-        uint16_t* dst = static_cast<uint16_t*>(p.shadow_t) + c * p.shadow_t_pitch + row0;
-        if (row0 + 32 <= p.M) {
-#pragma unroll
-          for (int t = 0; t < 4; ++t)
-            __stcs(reinterpret_cast<uint4*>(dst) + t, make_uint4(P[4 * t], P[4 * t + 1], P[4 * t + 2], P[4 * t + 3]));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (row0 + i < p.M) dst[i] = (uint16_t)((i & 1) ? (P[i >> 1] >> 16) : (P[i >> 1] & 0xffffu));
-        }
-      }
-    }
-#endif
-  }
-#endif  // AB_EP_STAGED
   __device__ __forceinline__ void finish_fullsum(const FF& acc, long long row, long long n0, int lane) const {
 #if AB_EP_FULLSUM >= 0
     double fs = ff_double(acc);
@@ -907,7 +689,7 @@ struct EpilogueOut {
     const int half_chunks = p.block_n >> 6;
     FF fs = {0.0f, 0.0f};
     ChunkPre pre;
-    prefetch_chunk(pre, row, n0, live, sc, lane);
+    prefetch_chunk(pre, row, n0, sc, lane);
 #pragma unroll 1
     for (int c = 0; c < nchunks; ++c) {
       float x[32];
@@ -918,8 +700,8 @@ struct EpilogueOut {
         __syncwarp();
         if (lane == 0) mbar_arrive(acc_free);
       }
-      if (c + 1 < nchunks) prefetch_chunk(pre, row, col0 + 32, live, sc, lane);
-      fused_reduce(x, row, col0, lane);
+      if (c + 1 < nchunks) prefetch_chunk(pre, row, col0 + 32, sc, lane);
+      fused_reduce(row, col0, lane);
       if ((c + 1) % half_chunks == 0) {
         finish_fullsum(fs, row, col0 + 32 - (p.block_n >> 1), lane);
         fs = FF{0.0f, 0.0f};
@@ -1094,7 +876,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
   const int stage_bytes = p.stage_bytes;
   const long long num_units = p.num_units;
   // persistent tile scheduler: CTA b handles units b, b + gridDim.x, ... (AB_UNIT_DECODE)
-  // behind the operand ring: the tile's float32 accumulator, then (AB_EP_STAGED) the epilogue's
+  // behind the operand ring: the tile's float32 accumulator, then (fused regions) the epilogue's
   // per-warp staging chunks
   const uint32_t acc_base = smem_u32(smem + (size_t)p.stages * p.stage_bytes);
   const uint32_t crank = CL > 1 ? cluster_ctarank() : 0u;  // position of this CTA along M
@@ -1191,7 +973,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
       const long long n0 = tile_n * p.block_n;
       // built per tile: held across the wait, the epilogue's state would cost the larger
       // generated regions their registers
-#if AB_EP_STAGED
+#ifdef AB_EPILOGUE
       const EpilogueOut eo(p, acc_base + kAccBytes + (uint32_t)(q * kStageBytesPerWarp));
 #else
       const EpilogueOut eo(p);
@@ -1219,9 +1001,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a0, const CUten
   if (CL > 1) cluster_sync_all();  // no CTA leaves while another may still multicast into it
 }
 
-#if AB_EP_STAGED
-extern "C" __global__ void ab_gemm_ep_staged_marker() {}  // tells gemm_run to reserve kStageBytes
-#endif
 #ifdef AB_EPILOGUE
 // NVRTC build: C-linkage entry points, one per MMA-loop layout (the module is loaded by name
 // from gemm_run, which picks the kernel of the packed operands' layout)

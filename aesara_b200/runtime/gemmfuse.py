@@ -121,7 +121,7 @@ class GemmEpilogueFusion:
         # the one value whose transposed bf16 plane the module can write (shares its registers
         # with the column sums, so it has to be that value when the region has column sums)
         cand = [k for k, v in enumerate(out_vars) if v is not None and _plane_users(program, v)[1]]
-        if os.environ.get("AB_EP_NO_TPLANE") or (self.fullsum >= 0 and os.environ.get("AB_EP_TPLANE_NO_FULLSUM")):
+        if os.environ.get("AB_EP_NO_TPLANE"):
             cand = []
         self.tplane = (self.colsum if self.colsum in cand else -1) if self.colsum >= 0 else (cand[0] if cand else -1)
         self.exact_sums = True                # set by the executor: float-pair sums (fp32-faithful policy)

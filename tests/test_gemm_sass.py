@@ -85,7 +85,7 @@ def test_ahead_of_time_gemm_kernels_keep_a_kblock_in_flight():
     lib.load()
     sass = subprocess.run(["cuobjdump", "-sass", build.lib_path()], capture_output=True, text=True, check=True).stdout
     kernels = {n: ev for n, ev in sass_functions(sass).items() if "gemm_tc_kernel" in n}
-    assert len(kernels) == 4, sorted(kernels)  # {tf32, bf16} x {single CTA, cluster of 4}
+    assert len(kernels) == 4, sorted(kernels)  # {tf32, bf16} x {single CTA, CTA pair}
     for name, ev in kernels.items():
         check_pipelined(name, ev)
 
@@ -103,8 +103,7 @@ def test_fused_epilogue_gemm_kernels_keep_a_kblock_in_flight(precision, monkeypa
     nvrtc = "%d.%d" % lib.nvrtc_version()
     for f in regions:
         cubin = lib.compile_cubin(f.source(), "gemm_ep")
-        kernels = {n: ev for n, ev in sass_functions(cubin_sass(cubin)).items() if n.startswith("ab_gemm_ep_")
-                   and "marker" not in n}
+        kernels = {n: ev for n, ev in sass_functions(cubin_sass(cubin)).items() if n.startswith("ab_gemm_ep_")}
         assert sorted(kernels) == sorted(EP_KERNELS)
         for name, ev in kernels.items():
             check_pipelined(f"{name} (region {f.g}, precision {precision}, NVRTC {nvrtc})", ev)

@@ -64,14 +64,15 @@ def test_gemm_fp32_faithful(K, m, n, k, layout):
 @pytest.mark.parametrize("layout", ["nn", "tn", "nt", "tt"])
 @pytest.mark.parametrize("m,n,k", [(1024, 256, 192), (1500, 520, 1000), (4096, 1024, 512), (2300, 256, 4160)])
 def test_gemm_four_cta_cluster_multicast(K, m, n, k, layout, precision, monkeypatch):
-    """With AB_GEMM_CLUSTER4 set, M >= 1024 takes the 4-CTA cluster kernel (four CTAs stacked along
-    M sharing the B tile: each loads a quarter and multicasts it to all four).  Its per-element
-    arithmetic is the single-CTA kernel's, so the result must be BIT-IDENTICAL to the default path
-    for every operand layout, ragged cluster tiles (trailing CTAs partly or wholly out of range)
-    and both the 3xTF32 and bf16 policies; and inside tolerance of a float64 product.  A
-    row-major B is packed K-major (transposing pack) by default; under the bf16 policy it is
-    also run with AB_GEMM_NO_TPACK, where it stays MN-major and each CTA multicasts its K rows
-    of every chunk."""
+    """CTA pairs, which replaced the 4-CTA cluster this test was written for (hence its name).
+    With AB_GEMM_CLUSTER=2 the product runs on CTA pairs (two CTAs stacked along M sharing the B
+    tile: each loads half of it and multicasts it to both), under the 3xTF32 policy too, where
+    pairs are not the default.  The per-element arithmetic is the single-CTA kernel's, so the
+    result must be BIT-IDENTICAL to AB_GEMM_CLUSTER=1 for every operand layout, ragged pair
+    tiles (the second CTA partly or wholly out of range) and both the 3xTF32 and bf16 policies;
+    and inside tolerance of a float64 product.  A row-major B is packed K-major (transposing
+    pack) by default; under the bf16 policy it is also run with AB_GEMM_NO_TPACK, where it
+    stays MN-major and each CTA multicasts its K rows of every chunk."""
     from collections import Counter
 
     rng = np.random.default_rng(m + n + k)
@@ -87,29 +88,28 @@ def test_gemm_four_cta_cluster_multicast(K, m, n, k, layout, precision, monkeypa
     for no_tpack in ((False, True) if precision == 2 else (False,)):
         if no_tpack:
             monkeypatch.setenv("AB_GEMM_NO_TPACK", "1")
-        # the variant is off by default (slower, see cluster_pairs)
-        monkeypatch.setenv("AB_GEMM_CLUSTER4", "1")
+        monkeypatch.setenv("AB_GEMM_CLUSTER", "2")
         before = Counter(K.TC_LAUNCHES)
-        C4 = _dev(c0)
-        K.gemm(C4, 0.8, A, B, 0.4, precision=precision)
-        b_mn = int(no_tpack and layout[1] == "n")
-        assert {key[3] for key, v in K.TC_LAUNCHES.items() if v > before[key]} == {b_mn}
-        monkeypatch.delenv("AB_GEMM_CLUSTER4")
         C2 = _dev(c0)
         K.gemm(C2, 0.8, A, B, 0.4, precision=precision)
-        got = C4.to_numpy()
-        np.testing.assert_array_equal(got, C2.to_numpy())
+        b_mn = int(no_tpack and layout[1] == "n")
+        assert {key[3] for key, v in K.TC_LAUNCHES.items() if v > before[key]} == {b_mn}
+        monkeypatch.setenv("AB_GEMM_CLUSTER", "1")
+        C1 = _dev(c0)
+        K.gemm(C1, 0.8, A, B, 0.4, precision=precision)
+        got = C2.to_numpy()
+        np.testing.assert_array_equal(got, C1.to_numpy())
         assert _normwise(got, want) < (1e-5 if precision == 0 else 2e-2)
 
 
 @pytest.mark.parametrize("layout", ["tn", "nt", "tt", "nn"])
 @pytest.mark.parametrize("m,n,k", [(512, 768, 640), (1024, 256, 200), (320, 576, 4160), (300, 520, 512)])
 def test_gemm_mn_major_tiles_as_one_bulk_copy(K, m, n, k, layout, monkeypatch):
-    """With AB_GEMM_MN3D set, bf16 MN-major operands (a matrix used transposed) arrive through a
-    3-D tensor map, one cp.async.bulk.tensor per tile, when the MN extent is a multiple of 64;
-    bit-identical to the default one-copy-per-chunk path, ragged extents keep that path.
+    """bf16 MN-major operands (a matrix used transposed) arrive as one 2-D copy per 128-byte chunk
+    of the MN index, whether the MN extent is a multiple of 64 or ragged.  (The name is that of
+    the 3-D single-copy variant this test once compared with; that variant is gone.)
     AB_GEMM_NO_TPACK keeps these small operands MN-major (they would get a transposing pack);
-    "nt" (both operands K-major) is the control that MN3D leaves alone."""
+    "nt" (both operands K-major) is the control."""
     from collections import Counter
 
     monkeypatch.setenv("AB_GEMM_NO_TPACK", "1")
@@ -123,19 +123,13 @@ def test_gemm_mn_major_tiles_as_one_bulk_copy(K, m, n, k, layout, monkeypatch):
         pass  # B [k, n] row-major is MN-major as it stands
     else:
         B = _dev(np.ascontiguousarray(b.T)).dimshuffle([1, 0])
-    monkeypatch.setenv("AB_GEMM_MN3D", "1")   # off by default (measured slower for MN-major A operands)
     before = Counter(K.TC_LAUNCHES)
-    C3 = _dev(np.zeros((m, n), "float32"))
-    K.gemm(C3, 1.0, A, B, 0.0, precision=2)
+    C = _dev(np.zeros((m, n), "float32"))
+    K.gemm(C, 1.0, A, B, 0.0, precision=2)
     want_key = (False, 2, int(layout[0] == "t"), int(layout[1] == "n"))
     assert [key for key, v in K.TC_LAUNCHES.items() if v > before[key]] == [want_key]
-    monkeypatch.delenv("AB_GEMM_MN3D")
-    C2 = _dev(np.zeros((m, n), "float32"))
-    K.gemm(C2, 1.0, A, B, 0.0, precision=2)
-    got = C3.to_numpy()
-    np.testing.assert_array_equal(got, C2.to_numpy())
     want = a.astype(np.float64) @ b.astype(np.float64)
-    assert _normwise(got, want) < 2e-2
+    assert _normwise(C.to_numpy(), want) < 2e-2
 
 
 @pytest.mark.parametrize("m,n,k", [(256, 256, 4096), (512, 256, 16384), (256, 512, 65536)])

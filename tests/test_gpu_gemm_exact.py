@@ -219,13 +219,15 @@ def test_exact_ring_and_unit_order(K, monkeypatch, knob, m, n, k, precision, la,
 @pytest.mark.parametrize("precision,la,lb", [(0, "k", "k"), (0, "mn", "mn"), (2, "k", "k"), (2, "k", "mn"),
                                               (2, "mn", "mn")])
 def test_exact_four_cta_cluster(K, monkeypatch, m, n, k, precision, la, lb):
-    """AB_GEMM_CLUSTER4 on a ragged M (trailing CTAs partly or wholly out of range) and on a
-    multi-unit shape (~128 cluster tiles for ~33 resident clusters), with K- and MN-major B
-    (per-chunk multicast): exact, and bit-identical to the single-CTA kernel."""
+    """CTA pairs, which replaced the 4-CTA cluster this test is named after.
+    AB_GEMM_CLUSTER=2 (CTA pairs, under the 3xTF32 policy too) on a ragged M (the second CTA of
+    the last pair partly or wholly out of range) and on a multi-unit shape (~256 pair tiles for
+    ~66 resident pairs), with K- and MN-major B (per-chunk multicast): exact, and bit-identical to
+    the single-CTA kernel (AB_GEMM_CLUSTER=1)."""
     monkeypatch.setenv("AB_GEMM_NO_TPACK", "1")
-    monkeypatch.setenv("AB_GEMM_CLUSTER4", "1")
-    got = exact_case(K, m, n, k, precision, la, lb, True, 1.0, -2.0, what=f"cluster {m}x{n}x{k} {la}/{lb}")
-    monkeypatch.delenv("AB_GEMM_CLUSTER4")
+    monkeypatch.setenv("AB_GEMM_CLUSTER", "2")
+    got = exact_case(K, m, n, k, precision, la, lb, True, 1.0, -2.0, what=f"pair {m}x{n}x{k} {la}/{lb}")
+    monkeypatch.setenv("AB_GEMM_CLUSTER", "1")
     single = exact_case(K, m, n, k, precision, la, lb, True, 1.0, -2.0)
     np.testing.assert_array_equal(got, single)
 
@@ -233,10 +235,9 @@ def test_exact_four_cta_cluster(K, monkeypatch, m, n, k, precision, la, lb):
 @pytest.mark.parametrize("m,n,k", [(512, 768, 640), (4096, 1152, 640), (1024, 256, 200), (300, 520, 512)])
 @pytest.mark.parametrize("la,lb", [("mn", "k"), ("k", "mn"), ("mn", "mn")])
 def test_exact_mn_major_3d_tiles(K, monkeypatch, m, n, k, la, lb):
-    """AB_GEMM_MN3D: MN-major bf16 tiles as one 3-D bulk copy where the MN extent is a multiple
-    of 64 (300 and 520 are not: those operands keep the per-chunk copies)."""
+    """MN-major bf16 tiles, one 2-D copy per 128-byte chunk, at MN extents that are multiples of
+    64 and at ragged ones (300, 520).  (Named after the 3-D single-copy variant, which is gone.)"""
     monkeypatch.setenv("AB_GEMM_NO_TPACK", "1")
-    monkeypatch.setenv("AB_GEMM_MN3D", "1")
     exact_case(K, m, n, k, 2, la, lb, True)
 
 

@@ -263,8 +263,8 @@ def test_gemm_epilogue_sources_follow_the_precision_policy(monkeypatch):
     """The generated GEMM-epilogue module depends on the executor's product policy: float-pair
     (float64-equivalent) sums and no transposed plane under the fp32-faithful default, float32
     tree sums and the transposed bf16 plane of a value whose consumer contracts over its rows
-    under the bf16 policy; bias rows are recognised statically; the shared-memory staged
-    epilogue is the default and can be switched off.  The bf16-policy kernels of the cfg3
+    under the bf16 policy (AB_EP_NO_TPLANE switches it off); bias rows are recognised
+    statically.  The bf16-policy kernels of the cfg3
     regions compile (NVRTC, no GPU) with at most a small stack frame (no spills in the chunk loop)."""
     import re
     import subprocess
@@ -288,14 +288,11 @@ def test_gemm_epilogue_sources_follow_the_precision_policy(monkeypatch):
         d = [defines(f.source()) for f in regions]
         assert [x["AB_EP_EXACT_SUMS"] for x in d] == [exact] * 3
         assert [x["AB_EP_TPLANE"] for x in d] == [tplane] * 3    # h, dout, dpre: each feeds a weight gradient
-        assert [x["AB_EP_STAGED"] for x in d] == ["1"] * 3
         assert [x["AB_EP_ROWMASK"] for x in d] == ["1", "1", "0"]  # b1, b2 are [1, N] rows; region 3 reads h
         assert [x["AB_EP_COLSUM"] for x in d] == ["-1", "0", "0"] and [x["AB_EP_FULLSUM"] for x in d] == ["-1", "1", "-1"]
-    monkeypatch.setenv("AB_EP_NO_STAGING", "1")
     monkeypatch.setenv("AB_EP_NO_TPLANE", "1")
     d = [defines(f.source()) for f in ProgramExecutor(prog, precision=2)._fusions]
-    assert {x["AB_EP_STAGED"] for x in d} == {"0"} and {x["AB_EP_TPLANE"] for x in d} == {"-1"}
-    monkeypatch.delenv("AB_EP_NO_STAGING")
+    assert {x["AB_EP_TPLANE"] for x in d} == {"-1"}
     monkeypatch.delenv("AB_EP_NO_TPLANE")
     # no spills in the kernels the default bench launches (cuobjdump -res-usage of the cached cubin)
     import shutil
