@@ -2,16 +2,19 @@
 // embedding-lookup gather and its scatter-add gradient).
 //
 // Reference: aesara/tensor/subtensor.py:1925 (AdvancedSubtensor1.perform :1953-1990:
-// x.take(i, axis=0), negative indices wrap, out-of-range -> IndexError) and :2128
+// x.take(i, axis=0), negative indices wrap, out-of-range -> IndexError), :2128
 // (AdvancedIncSubtensor1.perform: np.add.at(x, idx, y) — duplicates accumulate — or
-// x[idx] = y with set_instead_of_inc).
+// x[idx] = y with set_instead_of_inc, where the last occurrence of a row wins) and :2700
+// (AdvancedIncSubtensor with ignore_duplicates: out[idx] += y, i.e. x[d] + y[last occurrence]).
 //
 // Byte/integer work, HBM-bound: rows of `inner` contiguous elements are moved with the
 // widest aligned vector; x is viewed as [n_rows, inner], idx as int64[n_idx].
 // Out-of-range indices cannot raise from a kernel: they set a device flag that the host
 // reads after the launch (the reference's IndexError).  Scatter-add uses atomicAdd, so
 // for floating point the order in which duplicates are summed is not fixed (integer
-// results are exact; float results agree to rounding).
+// results are exact; float results agree to rounding).  The last-occurrence modes first
+// record, for every destination row, the largest r that names it (atomicMax into an int64
+// workspace of n_rows); the second pass then writes row r only where it is that winner.
 #include <algorithm>
 
 #include "ab_common.h"
@@ -48,21 +51,38 @@ gather_rows_kernel(const V* __restrict__ x, long long x_row_stride_v, const IDX*
   }
 }
 
-template <typename T, typename IDX, bool SET>
+// pass 1 of the last-occurrence modes: winner[dst] = the largest r with idx[r] == dst
+template <typename IDX>
+__global__ void __launch_bounds__(kThreads)
+last_occurrence_kernel(const IDX* __restrict__ idx, long long idx_stride, long long n_idx,
+                       long long n_rows, long long* __restrict__ winner, int* err) {
+  for (long long r = (long long)blockIdx.x * kThreads + threadIdx.x; r < n_idx;
+       r += (long long)gridDim.x * kThreads) {
+    const long long dst = wrap_index(idx[r * idx_stride], n_rows, err);
+    if (dst >= 0) atomicMax(&winner[dst], r);
+  }
+}
+
+// MODE: AB_SCATTER_ADD (atomic, every occurrence), AB_SCATTER_SET / AB_SCATTER_ADD_LAST (only
+// the occurrence recorded in `winner` writes its row, so plain stores suffice)
+template <typename T, typename IDX, int MODE>
 __global__ void __launch_bounds__(kThreads)
 scatter_rows_kernel(T* __restrict__ x, long long x_row_stride, const IDX* __restrict__ idx,
                     long long idx_stride, const T* __restrict__ y, long long y_row_stride,
                     long long y_col_stride, long long n_idx, long long n_rows, long long inner,
-                    int* err) {
+                    const long long* __restrict__ winner, int* err) {
   const long long total = n_idx * inner;
   for (long long t = (long long)blockIdx.x * kThreads + threadIdx.x; t < total;
        t += (long long)gridDim.x * kThreads) {
     const long long r = t / inner, c = t - r * inner;
     const long long dst = wrap_index(idx[r * idx_stride], n_rows, err);
     if (dst < 0) continue;
+    if (MODE != AB_SCATTER_ADD && winner[dst] != r) continue;
     const T v = y[r * y_row_stride + c * y_col_stride];
-    if (SET) x[dst * x_row_stride + c] = v;
-    else atomicAdd(&x[dst * x_row_stride + c], v);
+    T* out = &x[dst * x_row_stride + c];
+    if (MODE == AB_SCATTER_SET) *out = v;
+    else if (MODE == AB_SCATTER_ADD_LAST) *out = (T)(*out + v);
+    else atomicAdd(out, v);
   }
 }
 
@@ -81,21 +101,24 @@ __device__ __forceinline__ void atomic_add_small(T* addr, T v) {
   } while (old != assumed);
 }
 
-template <typename T, typename IDX, bool SET>
+template <typename T, typename IDX, int MODE>
 __global__ void __launch_bounds__(kThreads)
 scatter_rows_small_kernel(T* __restrict__ x, long long x_row_stride, const IDX* __restrict__ idx,
                           long long idx_stride, const T* __restrict__ y, long long y_row_stride,
                           long long y_col_stride, long long n_idx, long long n_rows,
-                          long long inner, int* err) {
+                          long long inner, const long long* __restrict__ winner, int* err) {
   const long long total = n_idx * inner;
   for (long long t = (long long)blockIdx.x * kThreads + threadIdx.x; t < total;
        t += (long long)gridDim.x * kThreads) {
     const long long r = t / inner, c = t - r * inner;
     const long long dst = wrap_index(idx[r * idx_stride], n_rows, err);
     if (dst < 0) continue;
+    if (MODE != AB_SCATTER_ADD && winner[dst] != r) continue;
     const T v = y[r * y_row_stride + c * y_col_stride];
-    if (SET) x[dst * x_row_stride + c] = v;
-    else atomic_add_small<T>(&x[dst * x_row_stride + c], v);
+    T* out = &x[dst * x_row_stride + c];
+    if (MODE == AB_SCATTER_SET) *out = v;  // byte / half-word stores leave the neighbours alone
+    else if (MODE == AB_SCATTER_ADD_LAST) *out = (T)(*out + v);
+    else atomic_add_small<T>(out, v);
   }
 }
 
@@ -130,22 +153,42 @@ int gather_impl(int itemsize, const void* x, long long x_row_stride, const void*
   return AB_OK;
 }
 
+template <typename T, typename IDX, bool SMALL, int MODE>
+void launch_scatter(unsigned grid, T* xp, long long x_row_stride, const IDX* ip, long long idx_stride,
+                    const T* yp, long long y_rs, long long y_cs, long long n_idx, long long n_rows,
+                    long long inner, const long long* winner, int* err, cudaStream_t st) {
+  if constexpr (SMALL)
+    scatter_rows_small_kernel<T, IDX, MODE><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, winner, err);
+  else
+    scatter_rows_kernel<T, IDX, MODE><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, winner, err);
+}
+
 template <typename T, typename IDX, bool SMALL>
-int scatter_impl(bool set, void* x, long long x_row_stride, const void* idx, long long idx_stride,
+int scatter_impl(int mode, void* x, long long x_row_stride, const void* idx, long long idx_stride,
                  const void* y, long long y_rs, long long y_cs, long long n_idx, long long n_rows,
-                 long long inner, int* err, cudaStream_t st) {
+                 long long inner, void* workspace, size_t workspace_bytes, int* err, cudaStream_t st) {
   if (n_idx == 0 || inner == 0) return AB_OK;
   const unsigned grid = grid_for(n_idx * inner);
   T* xp = static_cast<T*>(x);
   const T* yp = static_cast<const T*>(y);
   const IDX* ip = static_cast<const IDX*>(idx);
-  if constexpr (SMALL) {
-    if (set) scatter_rows_small_kernel<T, IDX, true><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, err);
-    else scatter_rows_small_kernel<T, IDX, false><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, err);
-  } else {
-    if (set) scatter_rows_kernel<T, IDX, true><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, err);
-    else scatter_rows_kernel<T, IDX, false><<<grid, kThreads, 0, st>>>(xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, err);
+  long long* winner = static_cast<long long*>(workspace);
+  if (mode != AB_SCATTER_ADD) {
+    const size_t need = (size_t)n_rows * sizeof(long long);
+    if (!workspace || workspace_bytes < need)
+      return fail(AB_ERR_INVALID, "scatter workspace too small: need %zu bytes, have %zu", need,
+                  workspace_bytes);
+    AB_CUDA(cudaMemsetAsync(winner, 0xff, need, st));  // -1: no occurrence
+    last_occurrence_kernel<IDX><<<grid_for(n_idx), kThreads, 0, st>>>(ip, idx_stride, n_idx, n_rows, winner, err);
+    g_launches++;
+    AB_CUDA(cudaGetLastError());
   }
+  if (mode == AB_SCATTER_SET)
+    launch_scatter<T, IDX, SMALL, AB_SCATTER_SET>(grid, xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, winner, err, st);
+  else if (mode == AB_SCATTER_ADD_LAST)
+    launch_scatter<T, IDX, SMALL, AB_SCATTER_ADD_LAST>(grid, xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, winner, err, st);
+  else
+    launch_scatter<T, IDX, SMALL, AB_SCATTER_ADD>(grid, xp, x_row_stride, ip, idx_stride, yp, y_rs, y_cs, n_idx, n_rows, inner, winner, err, st);
   g_launches++;
   AB_CUDA(cudaGetLastError());
   return AB_OK;
@@ -195,20 +238,27 @@ extern "C" int ab_take_rows(int itemsize, int idx_dtype, const void* x, int64_t 
   return check ? read_and_clear_flag(flag, st, "AdvancedSubtensor1") : AB_OK;
 }
 
+extern "C" int ab_scatter_rows_workspace_bytes(int mode, int64_t n_rows, size_t* bytes) {
+  if (!bytes) return fail(AB_ERR_INVALID, "null out pointer");
+  *bytes = mode == AB_SCATTER_ADD ? 0 : (size_t)std::max<int64_t>(n_rows, 0) * sizeof(long long);
+  return AB_OK;
+}
+
 // x[idx[r], :] (+)= y[r, :]   (y may broadcast: strides 0)
-extern "C" int ab_scatter_rows(int dtype, int idx_dtype, int set_instead_of_inc, void* x,
-                               int64_t x_row_stride, int64_t n_rows, int64_t inner,
-                               const void* idx, int64_t idx_stride, int64_t n_idx, const void* y,
-                               int64_t y_row_stride, int64_t y_col_stride, int check,
-                               void* stream) {
+extern "C" int ab_scatter_rows(int dtype, int idx_dtype, int mode, void* x, int64_t x_row_stride,
+                               int64_t n_rows, int64_t inner, const void* idx, int64_t idx_stride,
+                               int64_t n_idx, const void* y, int64_t y_row_stride,
+                               int64_t y_col_stride, void* workspace, size_t workspace_bytes,
+                               int check, void* stream) {
+  if (mode != AB_SCATTER_ADD && mode != AB_SCATTER_SET && mode != AB_SCATTER_ADD_LAST)
+    return fail(AB_ERR_INVALID, "bad scatter mode %d", mode);
   cudaStream_t st = as_stream(stream);
   int* flag = error_flag();
   if (!flag) return fail(AB_ERR_CUDA, "cannot allocate the index-error flag");
-  const bool set = set_instead_of_inc != 0;
   int rc = AB_ERR_UNSUPPORTED;
 #define AB_SC(T, SMALL)                                                                          \
-  (idx_dtype == AB_I64 ? scatter_impl<T, long long, SMALL>(set, x, x_row_stride, idx, idx_stride, y, y_row_stride, y_col_stride, n_idx, n_rows, inner, flag, st) \
-   : idx_dtype == AB_I32 ? scatter_impl<T, int, SMALL>(set, x, x_row_stride, idx, idx_stride, y, y_row_stride, y_col_stride, n_idx, n_rows, inner, flag, st)    \
+  (idx_dtype == AB_I64 ? scatter_impl<T, long long, SMALL>(mode, x, x_row_stride, idx, idx_stride, y, y_row_stride, y_col_stride, n_idx, n_rows, inner, workspace, workspace_bytes, flag, st) \
+   : idx_dtype == AB_I32 ? scatter_impl<T, int, SMALL>(mode, x, x_row_stride, idx, idx_stride, y, y_row_stride, y_col_stride, n_idx, n_rows, inner, workspace, workspace_bytes, flag, st)    \
                          : fail(AB_ERR_UNSUPPORTED, "index dtype code %d (int32/int64 supported)", idx_dtype))
   switch (dtype) {
     case AB_F32: rc = AB_SC(float, false); break;

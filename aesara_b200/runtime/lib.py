@@ -166,10 +166,12 @@ SIGNATURES = {
         [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64,
          C.c_int64, C.c_void_p, C.c_int, C.c_void_p],
     ),
+    "ab_scatter_rows_workspace_bytes": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "ab_scatter_rows": (
         C.c_int,
         [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p,
-         C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p],
+         C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_size_t, C.c_int,
+         C.c_void_p],
     ),
     "ab_cell_scan_supported": (C.c_int, [C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64]),
     "ab_cell_scan_workspace_bytes": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]),
@@ -239,6 +241,12 @@ def load():
                     f"libaesara_b200.so is missing and could not be built ({e}); the GPU "
                     "backend has no CPU fallback"
                 ) from e
+        # The library binds the first libnvrtc.so.12 in the process.  Importing torch first
+        # makes that torch's bundled NVRTC in every process, build() included: the cubins
+        # build() caches are then keyed (compile_cubin) on the NVRTC the tests and the bench
+        # use, instead of the toolkit's one, which no later process would find.
+        import torch  # noqa: F401
+
         lib = C.CDLL(path, mode=C.RTLD_GLOBAL)
         for name, (res, args) in SIGNATURES.items():
             try:

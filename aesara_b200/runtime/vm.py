@@ -1092,7 +1092,7 @@ def _advincsub(ex, i, node, args):
     rest = x.shape[k:]
     x2 = x.reshape_view((rows,) + rest)
     sub = Node("AdvancedIncSubtensor1", node.inputs[:3], node.outputs,
-               {"inplace": True, "set": p["set"]})
+               {"inplace": True, "set": p["set"], "ignore_duplicates": p.get("ignore_duplicates", False)})
     _EXEC["AdvancedIncSubtensor1"](ex, i, sub, [x2, y, flat])
     return x
 
@@ -1249,6 +1249,8 @@ def _arange(ex, i, node, args):
 
 @_op("AdvancedIncSubtensor1")
 def _advincsub1(ex, i, node, args):
+    import ctypes as C
+
     from ..ir import DTYPE_CODE
     from . import lib as _lib
     from .device import stream_handle
@@ -1284,11 +1286,19 @@ def _advincsub1(ex, i, node, args):
     yb = DeviceArray.empty(want, x.dtype)
     K.copy_into(yb, y)
     y_rs, y_cs = (inner, 1)
+    # set: the last occurrence of a row wins (x[idx] = y); ignore_duplicates (from
+    # AdvancedIncSubtensor): x[d] + y[last occurrence] (out[idx] += y); else np.add.at
+    mode = 1 if p["set"] else (2 if p.get("ignore_duplicates") else 0)
+    lib = _lib.load()
+    ws_bytes = C.c_size_t()
+    _lib.check(lib.ab_scatter_rows_workspace_bytes(mode, x.shape[0], C.byref(ws_bytes)))
+    ws = DeviceArray.empty((ws_bytes.value,), "uint8") if ws_bytes.value else None
     try:
-        _lib.check(_lib.load().ab_scatter_rows(DTYPE_CODE[x.dtype.name], DTYPE_CODE[idx.dtype.name],
-                                               1 if p["set"] else 0, x.ptr, row_stride, x.shape[0],
-                                               inner, idx.ptr, idx.strides[0], idx.shape[0], yb.ptr,
-                                               y_rs, y_cs, 1, stream_handle()))
+        _lib.check(lib.ab_scatter_rows(DTYPE_CODE[x.dtype.name], DTYPE_CODE[idx.dtype.name], mode,
+                                       x.ptr, row_stride, x.shape[0], inner, idx.ptr, idx.strides[0],
+                                       idx.shape[0], yb.ptr, y_rs, y_cs,
+                                       ws.ptr if ws is not None else None, ws_bytes.value, 1,
+                                       stream_handle()))
     except _lib.AbError as e:
         if e.code == 4:
             raise IndexError(str(e)) from None

@@ -247,17 +247,25 @@ int ab_max_and_argmax(int dtype, int64_t outer, int64_t r, const void* in, void*
 /* ---- integer-array indexing (SURVEY §8f N3) ---------------------------------------
  * ab_take_rows: AdvancedSubtensor1 (aesara/tensor/subtensor.py:1925): out[r,:] = x[idx[r],:]
  *   over x viewed as [n_rows, inner] (inner contiguous, rows x_row_stride elements apart);
- *   negative indices wrap.  ab_scatter_rows: AdvancedIncSubtensor1 (:2128):
- *   x[idx[r],:] += y[r,:] (duplicates accumulate, np.add.at) or = y[r,:].
+ *   negative indices wrap.  ab_scatter_rows: AdvancedIncSubtensor1 (:2128) and
+ *   AdvancedIncSubtensor (:2700), by mode:
+ *     AB_SCATTER_ADD       x[idx[r],:] += y[r,:] for every r (duplicates accumulate, np.add.at);
+ *     AB_SCATTER_SET       x[d,:] = y[r,:] with r the LAST occurrence of d in idx (x[idx] = y);
+ *     AB_SCATTER_ADD_LAST  x[d,:] += y[r,:], r the last occurrence (out[idx] += y, the
+ *                          reference's ignore_duplicates).
+ *   The last-occurrence modes need ab_scatter_rows_workspace_bytes (an int64 per row) of
+ *   workspace; AB_SCATTER_ADD needs none.
  * check != 0: synchronise and return AB_ERR_SHAPE if an index was out of range
  * (the reference's IndexError). */
+typedef enum { AB_SCATTER_ADD = 0, AB_SCATTER_SET = 1, AB_SCATTER_ADD_LAST = 2 } ab_scatter_mode;
 int ab_take_rows(int itemsize, int idx_dtype, const void* x, int64_t x_row_stride, int64_t n_rows,
                  int64_t inner, const void* idx, int64_t idx_stride, int64_t n_idx, void* out,
                  int check, void* stream);
-int ab_scatter_rows(int dtype, int idx_dtype, int set_instead_of_inc, void* x,
-                    int64_t x_row_stride, int64_t n_rows, int64_t inner, const void* idx,
-                    int64_t idx_stride, int64_t n_idx, const void* y, int64_t y_row_stride,
-                    int64_t y_col_stride, int check, void* stream);
+int ab_scatter_rows_workspace_bytes(int mode, int64_t n_rows, size_t* bytes);
+int ab_scatter_rows(int dtype, int idx_dtype, int mode, void* x, int64_t x_row_stride,
+                    int64_t n_rows, int64_t inner, const void* idx, int64_t idx_stride,
+                    int64_t n_idx, const void* y, int64_t y_row_stride, int64_t y_col_stride,
+                    void* workspace, size_t workspace_bytes, int check, void* stream);
 
 /* AdvancedSubtensor / AdvancedIncSubtensor with one integer vector per leading dimension
  * (x[i, j], aesara/tensor/subtensor.py:2577/2727): ab_ravel_index folds the k int64 index

@@ -32,6 +32,11 @@ def _compile_all(t):
         prog = load_case(n)[0]
         if any(nd.op in ("Dot22", "Gemm", "Dot22Scalar") for nd in prog.nodes):
             exs += [ProgramExecutor(prog, precision=pr) for pr in (1, 2)]
+    # the reduction signatures the kernel-edge tests cover beyond the fixtures
+    from tests.test_gpu_kernel_edges import REDUCE_SIGNATURES
+
+    for sig in REDUCE_SIGNATURES:
+        K.CAReduceKernel.get(*sig)
     kerns = list(K.ElemwiseKernel._by_key.values()) + list(K.CAReduceKernel._by_key.values())
     for dt in ("float32", "float64", "int64", "int32", "int8", "bool"):
         kerns.append(K._identity_kernel(dt))
