@@ -188,6 +188,34 @@ def test_generated_scan_cells_compile_for_sm90a():
         spec.compile()
 
 
+_SCAN_CELL_GRAPHS = [(name, "all") for name in ("G1S1hs0", "G3S1hs0", "G2S3hs1", "G4S2hs1_ch", "rnn_tanh",
+                                                 "gated", "lstm_hc", "lstm_ch")] + [
+    (name, v) for name in ("G1S1hs0", "G2S3hs1") for v in ("last", "backwards", "wt", "nsteps2")]
+
+
+@pytest.mark.parametrize("name,variant", _SCAN_CELL_GRAPHS, ids=[f"{n}-{v}" for n, v in _SCAN_CELL_GRAPHS])
+def test_scan_cell_graphs_of_the_device_suite_match_and_compile(name, variant):
+    """The Scan graphs of tests/test_gpu_scan_cell.py, built with the reference front end: the
+    matcher finds the expected (gates, states, recurrent state, LSTM) at every shape the suite
+    runs, and the generated cell compiles for sm_90a (NVRTC, no GPU)."""
+    from aesara_b200.compat import bootstrap
+
+    if not bootstrap.available():
+        pytest.skip("reference front-end (oracle/_ref) not present")
+    from aesara_b200.runtime.vm import ProgramExecutor
+    from tests import _scan_cells as SC
+
+    c = SC.CELLS[name]
+    ex = ProgramExecutor(SC.program(name, variant))
+    r = [st["runner"] for st in ex._state if "runner" in st][0]
+    assert r.cell is not None
+    for B, H in ((128, 64), (200, 128), (2048, 320), (8, 1088)):
+        spec = r.cell.match(B, H, c.G)
+        assert spec is not None, (B, H)
+        assert (spec.gates, spec.states, spec.hs, spec.is_lstm) == (c.G, c.S, c.hs, c.is_lstm)
+    spec.compile()
+
+
 # ---------------------------------------------------------------- executor-level regions
 def test_fusion_regions_detected_on_the_committed_programs():
     """Region detection is host logic over the lowered program: cfg5 has one row region
