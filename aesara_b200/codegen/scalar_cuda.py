@@ -188,8 +188,14 @@ def _invert(a, idt, odt, st):  # basic.py:1720-1725
 
 
 def _trunc(a, idt, odt, st):  # basic.py:2702
+    # the argument is cast to the output type first (trunc(int32) is float64), as in
+    # _unary_float: floor() of a raw integer is ambiguous, and the reference's -(x) of
+    # INT_MIN overflows where NumPy's trunc gives INT_MIN
+    if odt not in FLOATS:
+        raise UnsupportedScalar(f"trunc with output dtype {odt}")
     fl = _f("floor", odt)
-    return f"(({a[0]}) >= 0 ? {fl}({a[0]}) : -{fl}(-({a[0]})))"
+    x = f"(({ctype(odt)}){a[0]})"
+    return f"({x} >= 0 ? {fl}({x}) : -{fl}(-{x}))"
 
 
 def _float_only(fn_name):

@@ -50,7 +50,15 @@ int sm_count() {
   return n;
 }
 
+// launches per kernel flavour (Module::EW_*), so that callers can tell which one ran
+std::atomic<uint64_t> g_path_launches[Module::EW_TILE + 1];
+
 }  // namespace
+
+extern "C" uint64_t ab_elemwise_path_count(int which) {
+  if (which < 0 || which > Module::EW_TILE) return 0;
+  return g_path_launches[which].load(std::memory_order_relaxed);
+}
 
 extern "C" int ab_elemwise_launch(ab_module* mod, int n_in, int n_out, int ndim,
                                   const int64_t* shape, void* const* ptrs,
@@ -212,5 +220,6 @@ extern "C" int ab_elemwise_launch(ab_module* mod, int n_in, int n_out, int ndim,
   void* args[1] = {P.buf.data()};
   AB_CUDA(cudaLaunchKernel((const void*)kern, grid, dim3(threads), args, 0, as_stream(stream)));
   g_launches.fetch_add(1, std::memory_order_relaxed);
+  g_path_launches[which].fetch_add(1, std::memory_order_relaxed);
   return AB_OK;
 }

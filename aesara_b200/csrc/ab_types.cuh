@@ -27,10 +27,13 @@ typedef unsigned long long ab_u64;
 // aesara/scalar/basic.py:2055-2127 (FloorDivide) and :2165-2240 (Mod): the
 // reference raises ZeroDivisionError on the host for y == 0; a device kernel
 // cannot raise, it follows the reference's own `#ifdef KERNEL` branch (x / y,
-// x % y evaluated by the hardware) but returns 0 to stay defined.
+// x % y evaluated by the hardware) but returns 0 to stay defined.  y == -1 is answered
+// without dividing: MIN / -1 overflows (undefined in C++); NumPy gives MIN // -1 = MIN (the
+// negation wraps) and MIN % -1 = 0.
 template <typename T>
 __device__ __forceinline__ T ab_floordiv_int(T x, T y) {
   if (y == 0) return (T)0;
+  if (y == (T)-1) return (T)(0ULL - (unsigned long long)x);
   T q = x / y;
   T r = x % y;
   if ((r != 0) && ((r < 0) != (y < 0))) q -= 1;
@@ -38,7 +41,7 @@ __device__ __forceinline__ T ab_floordiv_int(T x, T y) {
 }
 template <typename T>
 __device__ __forceinline__ T ab_mod_int(T x, T y) {
-  if (y == 0) return (T)0;
+  if (y == 0 || y == (T)-1) return (T)0;
   T r = x % y;
   if ((r != 0) && ((r < 0) != (y < 0))) r += y;
   return r;
@@ -70,17 +73,33 @@ __device__ __forceinline__ double ab_floordiv_f(double x, double y) {
   return floor(x / y);
 }
 // Python-sign floating modulo (basic.py:2207-2236)
+// branch for branch, so that a zero remainder has the reference's sign (-6 % 3 = +0, not the
+// -0 of fmod(-6, 3))
 __device__ __forceinline__ float ab_mod_f(float x, float y) {
   if (y == 0.0f) return fmodf(x, y);
-  float r = fmodf(x, y);
-  if (r != 0.0f && ((r < 0.0f) != (y < 0.0f))) r += y;
-  return r;
+  if (y < 0.0f) {
+    if (x < 0.0f) return -fmodf(-x, -y);
+    const float m = fmodf(x, -y);
+    return m + (m != 0.0f ? y : 0.0f);
+  }
+  if (x < 0.0f) {
+    const float m = fmodf(-x, y);
+    return -m + (m != 0.0f ? y : 0.0f);
+  }
+  return fmodf(x, y);
 }
 __device__ __forceinline__ double ab_mod_f(double x, double y) {
   if (y == 0.0) return fmod(x, y);
-  double r = fmod(x, y);
-  if (r != 0.0 && ((r < 0.0) != (y < 0.0))) r += y;
-  return r;
+  if (y < 0.0) {
+    if (x < 0.0) return -fmod(-x, -y);
+    const double m = fmod(x, -y);
+    return m + (m != 0.0 ? y : 0.0);
+  }
+  if (x < 0.0) {
+    const double m = fmod(-x, y);
+    return -m + (m != 0.0 ? y : 0.0);
+  }
+  return fmod(x, y);
 }
 
 // ---- maximum / minimum with the reference's NaN rule (basic.py:1745-1752) ------

@@ -69,6 +69,7 @@ SIGNATURES = {
         [C.c_void_p, C.c_int, C.c_int, C.c_int, c_i64p, c_voidpp, c_i64p, c_i32p, C.c_int,
          C.c_int, C.c_void_p],
     ),
+    "ab_elemwise_path_count": (C.c_uint64, [C.c_int]),
     "ab_careduce_workspace_bytes": (
         C.c_int, [C.c_int, c_i64p, c_i32p, C.c_int, C.POINTER(C.c_size_t)]
     ),

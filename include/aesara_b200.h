@@ -113,6 +113,9 @@ int ab_kernel_launch(ab_module* m, const char* name, unsigned grid_x, unsigned b
 int ab_elemwise_launch(ab_module* m, int n_in, int n_out, int ndim, const int64_t* shape,
                        void* const* ptrs, const int64_t* strides, const int32_t* itemsizes,
                        int vec, int unroll, void* stream);
+/* Number of ab_elemwise_launch calls since load that ran kernel flavour `which`:
+ * 0 flat_vec, 1 flat, 2 rows_vec, 3 rows, 4 nd, 5 tile (0 for any other value). */
+uint64_t ab_elemwise_path_count(int which);
 
 /* ---- CAReduce (aesara/tensor/elemwise.py:1221, C loop elemwise_cgen.py:502) -
  * Reduce `in` over the axes flagged in reduce_mask into a C-contiguous `out`

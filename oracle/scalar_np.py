@@ -33,6 +33,32 @@ def _cast_like_c(x, dtype):
         return x.astype(dt)
 
 
+def _c_common(a, b):
+    """C's usual arithmetic conversions (the reference's C writes ``x < y``, ``x + y``,
+    ``c ? x : y`` on the typed operands): integer promotion to int first, then the wider type
+    of one signedness, an unsigned type over a signed one no wider than it, an int64 over a
+    uint32; a float over any integer (int64 with float32 is float32)."""
+    a, b = (np.dtype(np.int32) if (d.kind in "iub" and d.itemsize < 4) else d
+            for d in (np.dtype(a), np.dtype(b)))
+    if a.kind == "f" or b.kind == "f":
+        return np.dtype(np.float64) if np.dtype(np.float64) in (a, b) else np.dtype(np.float32)
+    if a.kind == b.kind or a == b:
+        return a if a.itemsize >= b.itemsize else b
+    signed, unsigned = (a, b) if a.kind == "i" else (b, a)
+    return unsigned if unsigned.itemsize >= signed.itemsize else signed
+
+
+def _c_pair(x, y):
+    x, y = np.asarray(x), np.asarray(y)
+    t = _c_common(x.dtype, y.dtype)
+    with np.errstate(**_ERR):
+        return x.astype(t), y.astype(t)
+
+
+def _c_where(c, x, y):  # c ? x : y
+    return np.where(np.asarray(c) != 0, *_c_pair(x, y))
+
+
 def _upgrade(x, out_dtype):
     """``exp((T)x)`` style ops cast the argument to the *output* type first
     (basic.py:3102-3109)."""
@@ -72,18 +98,33 @@ def _log1mexp(x):  # scalar/math.py:1248-1258
 
 def _py_mod(x, y):  # basic.py:2165-2240: result has the sign of y (Python %)
     with np.errstate(**_ERR):
-        if np.issubdtype(np.result_type(x, y), np.integer) or np.result_type(x, y) == np.bool_:
-            y_safe = np.where(y == 0, 1, y)
-            return np.where(y == 0, 0, np.mod(x, y_safe))
-        return np.mod(x, y)
+        rt = np.result_type(x, y)
+        if np.issubdtype(rt, np.integer) or rt == np.bool_:
+            x, y = np.asarray(x).astype(rt), np.asarray(y).astype(rt)
+            y_safe = np.where(y == 0, rt.type(1), y)
+            return np.where(y == 0, rt.type(0), np.mod(x, y_safe))
+        # floats: the reference's branches (basic.py:2222-2236), which give a zero remainder the
+        # sign np.mod does not (-6 % 3 = +0, 6 % -3 = +0)
+        rt = np.result_type(x, y)
+        x, y = np.broadcast_arrays(np.asarray(x, dtype=rt), np.asarray(y, dtype=rt))
+        zero = rt.type(0)
+        mm = -np.fmod(-x, -y)
+        pm = np.fmod(x, -y)
+        pm = pm + np.where(pm != 0, y, zero)
+        mp = np.fmod(-x, y)
+        mp = -mp + np.where(mp != 0, y, zero)
+        pp = np.fmod(x, y)
+        return np.where(y == 0, pp, np.where(y < 0, np.where(x < 0, mm, pm),
+                                             np.where(x < 0, mp, pp))).astype(rt)
 
 
 def _int_div(x, y):  # basic.py:2055-2127: floor division
     with np.errstate(**_ERR):
         rt = np.result_type(x, y)
         if np.issubdtype(rt, np.integer) or rt == np.bool_:
-            y_safe = np.where(y == 0, 1, y)
-            return np.where(y == 0, 0, np.floor_divide(x, y_safe))
+            x, y = np.asarray(x).astype(rt), np.asarray(y).astype(rt)
+            y_safe = np.where(y == 0, rt.type(1), y)
+            return np.where(y == 0, rt.type(0), np.floor_divide(x, y_safe))
         # floats: the reference divides magnitudes and corrects with fmod (basic.py:2083-2121);
         # this is not floor(x / y) for infinite divisors or when |x|/|y| rounds up to an integer
         x = np.asarray(x, dtype=rt)
@@ -127,19 +168,19 @@ def apply_op(st, args):
         if op == "add":  # basic.py:1829-1837 (bool: ||)
             r = a[0]
             for x in a[1:]:
-                r = np.logical_or(r, x) if out == np.bool_ else r + x
+                r = np.logical_or(r, x) if out == np.bool_ else np.add(*_c_pair(r, x))
         elif op == "mul":  # basic.py:1897-1907 (bool: &&)
             r = a[0]
             for x in a[1:]:
-                r = np.logical_and(r, x) if out == np.bool_ else r * x
+                r = np.logical_and(r, x) if out == np.bool_ else np.multiply(*_c_pair(r, x))
         elif op == "sub":  # :1955
-            r = a[0] - a[1]
+            r = np.subtract(*_c_pair(a[0], a[1]))
         elif op == "true_divide":  # :1997-2011 ((double)x / y for two discrete args)
             x, y = np.asarray(a[0]), np.asarray(a[1])
             if x.dtype.kind in "biu" and y.dtype.kind in "biu":
                 r = x.astype(np.float64) / y
             else:
-                r = x / y
+                r = np.true_divide(*_c_pair(x, y))
         elif op == "int_div":
             r = _int_div(a[0], a[1])
         elif op == "mod":
@@ -165,7 +206,7 @@ def apply_op(st, args):
         elif op in ("lt", "gt", "le", "ge", "eq", "neq"):
             fn = dict(lt=np.less, gt=np.greater, le=np.less_equal,
                       ge=np.greater_equal, eq=np.equal, neq=np.not_equal)[op]
-            r = fn(a[0], a[1])
+            r = fn(*_c_pair(a[0], a[1]))
         elif op == "isnan":
             r = np.isnan(a[0]) if np.asarray(a[0]).dtype.kind == "f" else np.zeros(np.shape(a[0]), bool)
         elif op == "isinf":
@@ -173,22 +214,23 @@ def apply_op(st, args):
         elif op == "inrange":
             lo = np.greater if st.get("openlow") else np.greater_equal
             hi = np.less if st.get("openhi") else np.less_equal
-            r = np.logical_and(lo(a[0], a[1]), hi(a[0], a[2]))
+            r = np.logical_and(lo(*_c_pair(a[0], a[1])), hi(*_c_pair(a[0], a[2])))
         elif op == "switch":  # :1586  cond ? a : b
-            r = np.where(np.asarray(a[0]) != 0, a[1], a[2])
+            r = _c_where(a[0], a[1], a[2])
         elif op == "clip":  # :2355
             x, lo, hi = a
-            r = np.where(x < lo, lo, np.where(x > hi, hi, x))
+            inner = _c_where(np.greater(*_c_pair(x, hi)), hi, x)
+            r = _c_where(np.less(*_c_pair(x, lo)), lo, inner)
         elif op == "maximum":
             r = _maximum(a[0], a[1])
         elif op == "minimum":
             r = _minimum(a[0], a[1])
         elif op == "or":
-            r = np.bitwise_or(a[0], a[1])
+            r = np.bitwise_or(*_c_pair(a[0], a[1]))
         elif op == "and":
-            r = np.bitwise_and(a[0], a[1])
+            r = np.bitwise_and(*_c_pair(a[0], a[1]))
         elif op == "xor":
-            r = np.bitwise_xor(a[0], a[1])
+            r = np.bitwise_xor(*_c_pair(a[0], a[1]))
         elif op == "invert":
             r = np.logical_not(a[0]) if out == np.bool_ else np.invert(a[0])
         elif op == "mean":
@@ -199,8 +241,8 @@ def apply_op(st, args):
             r = getattr(np, op)(_upgrade(a[0], out))
         elif op == "arctan2":
             r = np.arctan2(_upgrade(a[0], out), _upgrade(a[1], out))
-        elif op == "trunc":
-            r = np.trunc(a[0])
+        elif op == "trunc":  # of the argument cast to the float output: trunc(INT32_MIN) = -2**31
+            r = np.trunc(_upgrade(a[0], out))
         elif op == "round_half_to_even":
             r = np.rint(a[0])
         elif op == "round_half_away_from_zero":

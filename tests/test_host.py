@@ -400,3 +400,33 @@ def test_regions_can_be_switched_off(monkeypatch):
     for var in ("AB_NO_GEMM_FUSE", "AB_NO_RED_FUSE", "AB_NO_ROWFUSE"):
         monkeypatch.setenv(var, "1")
     assert not ProgramExecutor(prog)._fusions
+
+
+def test_host_eval_compares_with_the_device_c_conversions():
+    """The device bodies compare and combine typed operands under C's usual arithmetic
+    conversions (int32 with uint32 is uint32, int64 with uint64 is uint64, int64 with float32
+    is float32); host_eval, which answers the same expressions for small host operands, and the
+    oracle give the same values, so one program has one answer wherever it runs."""
+    from aesara_b200.runtime import host_eval
+    from oracle.scalar_np import eval_expr
+
+    def one(op, dts, out, vals):
+        expr = {"inputs": list(dts), "out_dtypes": [out], "outputs": ["t0"],
+                "stmts": [{"op": op, "args": [f"i{k}" for k in range(len(dts))], "dtype": out,
+                           "in_dtypes": list(dts)}]}
+        args = [np.asarray(v, dtype=d) for v, d in zip(vals, dts)]
+        assert host_eval.supports(expr)
+        h = host_eval.eval_expr(expr, args)[0]
+        o = eval_expr(expr, args)[0]
+        np.testing.assert_array_equal(h, o)
+        return h.item()
+
+    assert one("lt", ["int32", "uint32"], "bool", [-1, 5]) is False
+    assert one("gt", ["int64", "uint64"], "bool", [-1, 5]) is True
+    assert one("eq", ["int64", "float32"], "bool", [2 ** 24 + 1, 2 ** 24]) is True
+    assert one("lt", ["int16", "uint16"], "bool", [-1, 5]) is True  # both promote to int
+    assert one("add", ["int32", "uint32"], "int64", [-1, 0]) == 2 ** 32 - 1
+    assert one("or", ["int32", "uint32"], "int64", [-1, 0]) == 2 ** 32 - 1
+    assert one("switch", ["bool", "int32", "uint32"], "int64", [True, -1, 5]) == 2 ** 32 - 1
+    assert one("clip", ["int32", "uint32", "uint32"], "int64", [-1, 2, 9]) == 9
+    assert one("true_divide", ["int64", "float32"], "float64", [2 ** 24 + 1, 1.0]) == 2.0 ** 24
