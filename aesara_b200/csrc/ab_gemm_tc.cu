@@ -477,6 +477,8 @@ int gemm_run(int precision, long long M, long long N, long long K, float alpha,
   p.alpha = alpha; p.beta = beta;
   p.C = C; p.c_rs = c_rs; p.c_cs = c_cs;
   p.Cin = Cin ? Cin : C; p.cin_rs = Cin ? cin_rs : c_rs; p.cin_cs = Cin ? cin_cs : c_cs;
+  // a fused epilogue may leave C unwritten (C == nullptr); beta*C_in then needs its own matrix
+  if (beta != 0.0f && !p.Cin) return fail(AB_ERR_INVALID, "beta != 0 needs C_in (or C)");
   p.block_n = BLOCK_N;
   p.nparts = parts;
   p.k_elems_per_row = SW_BYTES / es;          // K elements per stage (64 bf16 / 32 tf32)

@@ -386,6 +386,11 @@ class GemmEpilogueFusion:
             store = not ((shadow or tshadow) and self._plane_only_ok(ex, env, v, (M, N)))
             plan.append((store, shadow, tshadow))
         req = EpilogueRequest(self, ops, plan, self.colsum >= 0, self.fullsum >= 0)
+        # buffers the members rewrite in place (the z of an in-place Gemm): packs of their old
+        # contents must not serve the products that read the region's values from that memory
+        destroyed = [env.get(nodes[m].inputs[p]) for m in self.members for p in ex._destroys[m]
+                     if p < len(nodes[m].inputs)]
+        destroyed = [d for d in destroyed if isinstance(d, DeviceArray)]
         ex._gemm_epilogue = req
         try:
             out = _EXEC[gn.op](ex, self.g, gn, gargs)
@@ -396,6 +401,9 @@ class GemmEpilogueFusion:
             return False
         finally:
             ex._gemm_epilogue = None
+        # before the planes of the new values are adopted (they may live at the same address)
+        for d in destroyed:
+            ex.pack_cache.invalidate(d.owner)
         if not req.applied:
             # the product took another path (SIMT / too small): finish node by node
             env[gn.outputs[0]] = out

@@ -390,6 +390,10 @@ def gemm(C_: DeviceArray, alpha, A: DeviceArray, B: DeviceArray, beta, precision
         TC_LAUNCHES[(epilogue is not None, precision, opa.mn_major, opb.mn_major)] += 1
         cin_args = (None, 0, 0) if cin is None else (cin.ptr, cin.strides[0], cin.strides[1])
         if epilogue is not None:
+            if cin is None:
+                # in place (C_ holds z): value 0 may be kept as a bf16 plane only, with C left
+                # unwritten, so beta*z is read through C_in
+                cin_args = (C_.ptr, C_.strides[0], C_.strides[1])
             ep = _lib.GemmEpilogue()
             ep.module = epilogue.fusion.handle()
             ep.n_operands = len(epilogue.operands)

@@ -273,6 +273,88 @@ def test_fusion_regions_detected_on_the_committed_programs():
         assert not [f for f in ProgramExecutor(prog)._fusions if type(f).__name__ == "RowFusion"]
 
 
+def _fused_region_names(kind):
+    from tests import _fused_regions as FR
+
+    return list(FR.GEMM if kind == "gemm" else FR.ROW)
+
+
+@pytest.mark.parametrize("name", _fused_region_names("gemm"))
+def test_fused_region_catalogue_detects_and_compiles(name, monkeypatch):
+    """The GEMM-epilogue graphs of tests/test_gpu_fused_regions.py, built with the reference front
+    end: each is one region with the member ops and ``#define``s the catalogue names under every
+    precision policy (a region with more than it takes keeps its largest legal prefix), and the
+    generated module compiles for sm_90a (NVRTC, no GPU)."""
+    from aesara_b200.compat import bootstrap
+
+    if not bootstrap.available():
+        pytest.skip("reference front-end (oracle/_ref) not present")
+    from aesara_b200.runtime.vm import ProgramExecutor
+    from tests import _fused_regions as FR
+
+    monkeypatch.setenv("AB_GEMM_FUSE_FP32", "1")
+    case = FR.GEMM[name]
+    prog = FR.gemm_program(name)
+    for precision in (0, 1, 2):
+        fs = [f for f in ProgramExecutor(prog, precision=precision)._fusions
+              if type(f).__name__ == "GemmEpilogueFusion"]
+        assert len(fs) == 1, f"{name} precision {precision}: {len(fs)} regions"
+        f = fs[0]
+        d = FR.defines(f.source())
+        assert d["AB_EP_EXACT_SUMS"] == (precision == 0)
+        if case.expect["defines"] is not None:
+            want = dict(case.expect["defines"], **({} if precision == 2 else {"AB_EP_TPLANE": -1}))
+            assert {k: d[k] for k in want} == want, f"precision {precision}"
+            assert [prog.nodes[m].op for m in f.members] == case.expect["ops"]
+        later = [i for i, n in enumerate(prog.nodes) if i > f.g and n.op in ("Elemwise", "CAReduce")]
+        assert len(later) - (len(f.members) - 1) == case.expect["left_out"]
+        assert f.compile_all() == 1
+
+
+@pytest.mark.parametrize("name", _fused_region_names("row"))
+def test_row_region_catalogue_detects_and_compiles(name):
+    """The row-region graphs of the same suite: one region each (two Gemv, the per-row Elemwise
+    and the Sums), and its module compiles for sm_90a at every register blocking J = 1..8."""
+    from aesara_b200.compat import bootstrap
+
+    if not bootstrap.available():
+        pytest.skip("reference front-end (oracle/_ref) not present")
+    from aesara_b200.runtime import lib
+    from aesara_b200.runtime.vm import ProgramExecutor
+    from tests import _fused_regions as FR
+
+    prog = FR.row_program(name)
+    (f,) = [f for f in ProgramExecutor(prog)._fusions if type(f).__name__ == "RowFusion"]
+    ops = [prog.nodes[i].op for i in f.members]
+    assert ops.count("Gemv") == 2 and ops.count("CAReduce") == len(f.sums) and f.g2 is not None
+    assert len(f.sums) == {"sums0": 0, "sums2": 2}.get(name, 1)
+    classes = tuple("scal" if prog.vars[v].ndim == 0 or prog.vars[v].const is not None else "row" for v in f.ext)
+    by_ptr = tuple(prog.vars[v].ndim == 0 and prog.vars[v].const is None for v in f.ext)
+    for J in range(1, 9):
+        lib.compile_cubin(f._module(J, classes, by_ptr)["src"], "rowfuse")
+
+
+def test_fused_gemm_refuses_beta_without_c_in():
+    """``ab_gemm_packed_fused`` with beta != 0 and neither C nor C_in (a value kept as a bf16
+    plane only) is an invalid call, refused before anything is launched."""
+    import ctypes as C
+
+    from aesara_b200.runtime import lib
+
+    L = lib.load()
+    M, N, K = 256, 256, 256
+    A = lib.GemmOperand(16, None, M, K, K, 0, 2)
+    B = lib.GemmOperand(16, None, N, K, K, 0, 2)
+    ep = lib.GemmEpilogue()
+    ep.module = 16
+    ep.n_operands = 0
+    ep.n_outputs = 1
+    rc = L.ab_gemm_packed_fused(2, M, N, K, 1.0, C.byref(A), C.byref(B), 1.0, None, 0, 0, None, N, 1,
+                                C.byref(ep), None)
+    assert rc == 3  # AB_ERR_INVALID
+    assert "C_in" in L.ab_last_error().decode()
+
+
 def test_fused_kernel_sources_compile_for_sm90a():
     """NVRTC (no GPU needed): the row-region kernel, the wgmma GEMM with a generated
     epilogue, and the reduction with a fused pre-map."""
