@@ -8,6 +8,7 @@
 #include <cstring>
 #include <map>
 #include <string>
+#include <vector>
 
 #include "../../include/aesara_b200.h"
 
@@ -16,6 +17,14 @@ namespace ab {
 std::string& last_error();
 int fail(int code, const char* fmt, ...);
 extern std::atomic<uint64_t> g_launches;
+
+// The Elemwise launcher's dimension collapse (ab_elemwise_launch.cpp), shared with every launcher
+// that walks several strided operands over one index space: drop size-1 dims, order the rest by
+// |stride| of operand `order_by` (largest first, stable), and merge neighbours that are jointly
+// contiguous for every operand.  strides[k*ndim + d] is operand k's stride along dim d; on return
+// shp holds the merged extents and st[k] operand k's strides along them.
+void collapse_dims(int nops, int ndim, const int64_t* shape, const int64_t* strides, int order_by,
+                   std::vector<int64_t>& shp, std::vector<std::vector<int64_t>>& st);
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 

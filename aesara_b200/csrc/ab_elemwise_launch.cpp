@@ -55,48 +55,24 @@ std::atomic<uint64_t> g_path_launches[Module::EW_TILE + 1];
 
 }  // namespace
 
-extern "C" uint64_t ab_elemwise_path_count(int which) {
-  if (which < 0 || which > Module::EW_TILE) return 0;
-  return g_path_launches[which].load(std::memory_order_relaxed);
-}
+namespace ab {
 
-extern "C" int ab_elemwise_launch(ab_module* mod, int n_in, int n_out, int ndim,
-                                  const int64_t* shape, void* const* ptrs,
-                                  const int64_t* strides, const int32_t* itemsizes, int vec,
-                                  int unroll, void* stream) {
-  Module* m = reinterpret_cast<Module*>(mod);
-  const int nops = n_in + n_out;
-  if (!m) return fail(AB_ERR_INVALID, "null module");
-  if (nops <= 0 || nops > AB_MAX_OPERANDS || n_out <= 0)
-    return fail(AB_ERR_INVALID, "bad operand count %d in / %d out", n_in, n_out);
-  if (ndim < 0 || ndim > AB_MAX_RAW_DIMS) return fail(AB_ERR_INVALID, "bad ndim %d", ndim);
-  if (vec < 1 || unroll < 1) return fail(AB_ERR_INVALID, "bad vec/unroll");
-
+void collapse_dims(int nops, int ndim, const int64_t* shape, const int64_t* strides, int order_by,
+                   std::vector<int64_t>& shp, std::vector<std::vector<int64_t>>& st) {
   // 1. squeeze
-  std::vector<int64_t> shp;
-  std::vector<std::vector<int64_t>> st(nops);
-  long long total = 1;
-  for (int d = 0; d < ndim; ++d) {
-    if (shape[d] < 0) return fail(AB_ERR_INVALID, "negative dimension");
-    total *= shape[d];
-  }
-  if (total == 0) return AB_OK;  // nothing to compute (elemwise.py:738-746)
+  shp.clear();
+  st.assign(nops, {});
   for (int d = 0; d < ndim; ++d) {
     if (shape[d] == 1) continue;
     shp.push_back(shape[d]);
     for (int k = 0; k < nops; ++k) st[k].push_back(strides[(size_t)k * ndim + d]);
   }
   int nd = (int)shp.size();
-  // outputs must not be broadcast
-  for (int k = n_in; k < nops; ++k)
-    for (int d = 0; d < nd; ++d)
-      if (st[k][d] == 0) return fail(AB_ERR_INVALID, "output operand %d has a broadcast stride", k - n_in);
-
-  // 2. order dims by |stride| of the first output, largest first (stable)
+  // 2. order dims by |stride| of operand `order_by`, largest first (stable)
   if (nd > 1) {
     std::vector<int> perm(nd);
     for (int d = 0; d < nd; ++d) perm[d] = d;
-    const std::vector<int64_t>& os = st[n_in];
+    const std::vector<int64_t>& os = st[order_by];
     std::stable_sort(perm.begin(), perm.end(),
                      [&](int a, int b) { return std::llabs(os[a]) > std::llabs(os[b]); });
     std::vector<int64_t> shp2(nd);
@@ -122,6 +98,42 @@ extern "C" int ab_elemwise_launch(ab_module* mod, int n_in, int n_out, int ndim,
       --nd;
     }
   }
+}
+
+}  // namespace ab
+
+extern "C" uint64_t ab_elemwise_path_count(int which) {
+  if (which < 0 || which > Module::EW_TILE) return 0;
+  return g_path_launches[which].load(std::memory_order_relaxed);
+}
+
+extern "C" int ab_elemwise_launch(ab_module* mod, int n_in, int n_out, int ndim,
+                                  const int64_t* shape, void* const* ptrs,
+                                  const int64_t* strides, const int32_t* itemsizes, int vec,
+                                  int unroll, void* stream) {
+  Module* m = reinterpret_cast<Module*>(mod);
+  const int nops = n_in + n_out;
+  if (!m) return fail(AB_ERR_INVALID, "null module");
+  if (nops <= 0 || nops > AB_MAX_OPERANDS || n_out <= 0)
+    return fail(AB_ERR_INVALID, "bad operand count %d in / %d out", n_in, n_out);
+  if (ndim < 0 || ndim > AB_MAX_RAW_DIMS) return fail(AB_ERR_INVALID, "bad ndim %d", ndim);
+  if (vec < 1 || unroll < 1) return fail(AB_ERR_INVALID, "bad vec/unroll");
+
+  long long total = 1;
+  for (int d = 0; d < ndim; ++d) {
+    if (shape[d] < 0) return fail(AB_ERR_INVALID, "negative dimension");
+    total *= shape[d];
+  }
+  if (total == 0) return AB_OK;  // nothing to compute (elemwise.py:738-746)
+  std::vector<int64_t> shp;
+  std::vector<std::vector<int64_t>> st;
+  collapse_dims(nops, ndim, shape, strides, n_in, shp, st);
+  int nd = (int)shp.size();
+  // outputs must not be broadcast
+  for (int k = n_in; k < nops; ++k)
+    for (int d = 0; d < nd; ++d)
+      if (st[k][d] == 0) return fail(AB_ERR_INVALID, "output operand %d has a broadcast stride", k - n_in);
+
   if (nd > AB_MAX_DIMS)
     return fail(AB_ERR_UNSUPPORTED, "Elemwise over %d non-mergeable dims (max %d)", nd, AB_MAX_DIMS);
   if (nd == 0) {  // a single element

@@ -14,6 +14,8 @@ schedule order and the first disagreement is reported with the Apply node that p
 
 from __future__ import annotations
 
+import copy
+
 import numpy as np
 
 from .compat.bootstrap import load_aesara
@@ -86,7 +88,9 @@ def check_function(inputs, outputs, values, mode=None, reference_linker="py", rt
     # B200 trace: every node's outputs, copied to the host when the node has run
     for c, v in zip(vm.input_storage, values):
         c[0] = np.array(_as_host(v), copy=True) if not np.isscalar(v) else v
-    all_inputs = [np.array(_as_host(c[0]), copy=True) for c in vm.input_storage]
+    # a Generator (random variables) is copied as it is before the B200 run advances it
+    all_inputs = [copy.deepcopy(c[0]) if isinstance(c[0], np.random.Generator)
+                  else np.array(_as_host(c[0]), copy=True) for c in vm.input_storage]
     for c, v in zip(ref_in, all_inputs):  # explicit inputs first, then shared variables
         c.storage[0] = v
     trace = {}
@@ -98,8 +102,25 @@ def check_function(inputs, outputs, values, mode=None, reference_linker="py", rt
     finally:
         ex.trace = prev
 
+    program = getattr(vm.executor, "program", None)
     report = []
     for pos, (node, thunk) in enumerate(zip(order, ref_thunks)):
+        if program is not None and program.nodes[pos].op == "RandomVariable" and pos in trace:
+            # the device does not draw the reference's NumPy stream: its sample is checked
+            # against the NumPy restatement of the device stream, then handed to the
+            # reference's cells so that the nodes downstream are compared like for like
+            msg, err = _check_random(program.nodes[pos], thunk, trace[pos])
+            thunk()
+            thunk.outputs[0][0] = copy.deepcopy(trace[pos][0])
+            thunk.outputs[1][0] = trace[pos][1]
+            if msg is not None:
+                text = f"node {pos} {node} output 1: {msg}"
+                if raise_on_mismatch:
+                    raise DualRunMismatch(pos, node, 1, err, text)
+                report.append((pos, node, text))
+            else:
+                report.append((pos, node, err))
+            continue
         thunk()
         if pos not in trace:
             continue  # executed inside a fused region: compared at the region's outputs
@@ -118,3 +139,40 @@ def check_function(inputs, outputs, values, mode=None, reference_linker="py", rt
         else:
             report.append((pos, node, 0.0 if not thunk.outputs else err))
     return report
+
+
+# float32 / float64 Box-Muller draws against the long-double truth from the same words: the
+# device's logf / sqrtf / sincospif and their float64 twins, plus the affine step
+_NORMAL_TOL = {"float32": 4e-6, "float64": 1e-14}
+
+
+def _check_random(pnode, thunk, traced):
+    """(message or None, error) of a RandomVariable node's device sample: uniform and
+    Bernoulli draws must equal the NumPy restatement of the stream (oracle/random_np.py) bit
+    for bit, normal draws must lie within ``_NORMAL_TOL * (1 + |truth|)`` of it.  The key is
+    the one the device drew: one full-range uint64 from the node's input Generator."""
+    from oracle.random_np import random_sample, random_shape
+
+    p = pnode.params
+    rng, size, _dtype, *params = [c[0] for c in thunk.inputs]
+    params = params[-1:] if p["dist"] == "bernoulli" else params
+    key = int(copy.deepcopy(rng).integers(0, 2 ** 64, dtype=np.uint64))
+    want = random_sample(p["dist"], p["dtype"], key, random_shape(size, params), params)
+    got = np.asarray(traced[1])
+    if got.shape != want.shape or got.dtype != np.dtype(p["dtype"]):
+        return f"sample {got.dtype}{got.shape} != {p['dtype']}{want.shape}", np.inf
+    state = traced[0].bit_generator.state
+    g = copy.deepcopy(rng)
+    g.integers(0, 2 ** 64, dtype=np.uint64)
+    if state != g.bit_generator.state:
+        return "the Generator did not advance by exactly one 64-bit draw", np.inf
+    if p["dist"] == "normal":
+        with np.errstate(invalid="ignore"):
+            err = np.abs(got.astype(np.float64) - want) / (1 + np.abs(want))
+        err = float(np.nanmax(err)) if err.size else 0.0
+        if not err <= _NORMAL_TOL[p["dtype"]]:
+            return f"normal draws off the stream by {err:.3g} (bound {_NORMAL_TOL[p['dtype']]:.0e})", err
+        return None, err
+    bad = int(np.sum(~((got == want) | (np.isnan(got) & np.isnan(want))) if got.dtype.kind == "f"
+                     else got != want))
+    return (f"{bad} draws differ from the stream" if bad else None), float(bad)

@@ -555,6 +555,46 @@ def _l_split(op, apply):
     return "Split", {"len_splits": int(op.len_splits)}
 
 
+# -- random variables ------------------------------------------------------------------
+# RandomVariable (aesara/tensor/random/op.py:344 perform): inputs (rng, size, dtype, *params),
+# outputs (rng_out, sample).  The device draws from its own Philox stream keyed by one 64-bit
+# draw of the node's Generator (runtime/vm.py, csrc/ab_random.cu); the Generator stays a host
+# value.  Distribution class -> (device distribution, output dtypes it draws).
+_RV_DISTS = {
+    "UniformRV": ("uniform", ("float32", "float64")),
+    "NormalRV": ("normal", ("float32", "float64")),
+    "BernoulliRV": ("bernoulli", ("int64",)),
+    "BinomialRV": ("bernoulli", ("int64",)),
+}
+
+
+@lowers("RandomVariable")
+def _l_random_variable(op, apply):
+    from aesara.graph.basic import Constant
+    from aesara.tensor.random.type import RandomGeneratorType
+
+    cls = type(op).__name__
+    name = getattr(op, "name", cls)
+    what = f"B200 backend: random variable {name} ({cls})"
+    hit = _RV_DISTS.get(cls)
+    if hit is None:
+        raise UnsupportedOp(f"{what} has no device implementation (device draws: uniform, normal, "
+                            "bernoulli, binomial with n = 1); there is no CPU fallback for tensor work")
+    if not isinstance(apply.inputs[0].type, RandomGeneratorType):
+        raise UnsupportedOp(f"{what}: the rng is a {apply.inputs[0].type}; the device draws from "
+                            "numpy Generator rngs only (RandomStream, not RandomState)")
+    dist, dtypes = hit
+    out_dtype = apply.outputs[1].type.dtype
+    if out_dtype not in dtypes:
+        raise UnsupportedOp(f"{what}: no device draw of dtype {out_dtype}")
+    if cls == "BinomialRV":
+        n = apply.inputs[3]
+        if not (isinstance(n, Constant) and np.all(np.asarray(n.data) == 1)):
+            raise UnsupportedOp(f"{what}: the device draws binomial variables with the constant n = 1 "
+                                "(Bernoulli) only")
+    return "RandomVariable", {"dist": dist, "dtype": out_dtype, "inplace": bool(op.inplace)}
+
+
 # -- Scan --------------------------------------------------------------------------------
 def optimized_inner_fgraph(op):
     """The inner graph of a ``Scan`` as the reference would *execute* it.

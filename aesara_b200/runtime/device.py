@@ -129,7 +129,8 @@ class DeviceArray:
         res, waits = [], False
         for v in values:
             if not isinstance(v, DeviceArray):
-                res.append(np.asarray(v))
+                # host values; a random variable's Generator is returned as it is
+                res.append(v if isinstance(v, np.random.Generator) else np.asarray(v))
                 continue
             if v.nbytes < PINNED_MIN_BYTES:
                 res.append(v.to_numpy())

@@ -10,8 +10,9 @@ into a CUDA graph keyed on the input buffers' (pointer, shape, strides) and
 replays it with a single ``cudaGraphLaunch``.
 
 Capturable = no device→host read while evaluating (no ``ScalarFromTensor`` /
-``Assert`` on device data, no ``as_while`` Scan).  Such programs transparently
-fall back to eager execution.  Host-side shape arithmetic is evaluated at
+``Assert`` on device data, no ``as_while`` Scan) and no random variable: a replay would
+reuse the key its capture drew from the Generator, so every replay would repeat the same
+draws.  Such programs transparently fall back to eager execution.  Host-side shape arithmetic is evaluated at
 capture time; a change of any input shape/pointer produces a new capture.
 The returned output arrays are owned by the captured graph and are overwritten
 by the next replay.
@@ -33,7 +34,9 @@ class GraphReplay:
         self.ex = executor
         self.max_graphs = max_graphs
         self._graphs = {}
-        self._uncapturable = False
+        # random variables draw a fresh key from their Generator on every call (runtime/vm.py)
+        prog = getattr(executor, "program", None)
+        self._uncapturable = prog is not None and any(n.op == "RandomVariable" for n in prog.nodes)
         self.replays = 0
 
     @staticmethod

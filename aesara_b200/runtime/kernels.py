@@ -161,6 +161,13 @@ def contiguous_copy(a: DeviceArray, order="C") -> DeviceArray:
     return out
 
 
+def cast_copy(a: DeviceArray, dtype) -> DeviceArray:
+    """A C-contiguous copy of ``a`` in ``dtype`` (C conversion, like ``ndarray.astype``)."""
+    out = DeviceArray.empty(a.shape, dtype)
+    copy_into(out, a)
+    return out
+
+
 def add_into(dst: DeviceArray, src: DeviceArray):
     """dst[...] += src (IncSubtensor without set_instead_of_inc)."""
     dt = dst.dtype.name

@@ -162,6 +162,11 @@ SIGNATURES = {
         C.c_int,
         [C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     ),
+    "ab_random": (
+        C.c_int,
+        [C.c_int, C.c_int, C.c_uint64, C.c_int, c_i64p, C.c_int, c_voidpp, c_i64p, C.c_void_p, C.c_int,
+         C.c_void_p],
+    ),
     "ab_take_rows": (
         C.c_int,
         [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64,

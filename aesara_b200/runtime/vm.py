@@ -14,6 +14,7 @@ implementation raises ``NotImplementedError`` at construction time.
 
 from __future__ import annotations
 
+import copy
 import os
 
 import numpy as np
@@ -74,6 +75,9 @@ _HOST_SLOTS = {
     "IncSubtensor": ("from", 2), "Assert": ("from", 1),
     "Reshape": (1,), "Join": (0,), "Split": (1, 2), "Gemm": (1, 4), "Gemv": (1, 4), "Ger": (1,),
     "Dot22Scalar": (2,), "IfElse": (0,),
+    # the Generator, the size and the dtype code of a random variable (the draws' key is taken
+    # from the Generator on the host, lower.py)
+    "RandomVariable": (0, 1, 2),
 }
 # node kinds through which "needed on the host" propagates from an output to the inputs (the
 # value is *computed* from them); Shape/Shape_i read only metadata and stop the propagation
@@ -478,7 +482,9 @@ class ProgramExecutor:
             if self.trace is not None:
                 vals = [env[v] for v in node.outputs]
                 self.trace[i] = [v.to_numpy() if isinstance(v, DeviceArray)
-                                 else (None if v is None or isinstance(v, slice) else np.array(v, copy=True))
+                                 else (None if v is None or isinstance(v, slice)
+                                       else copy.deepcopy(v) if isinstance(v, np.random.Generator)
+                                       else np.array(v, copy=True))
                                  for v in vals]
             for v in self._free_after[i]:
                 env.pop(v, None)
@@ -798,6 +804,13 @@ def _ger(ex, i, node, args):
 @_op("Dot")
 def _dot(ex, i, node, args):
     x, y = _as_dev_inputs(ex, i, node, args)
+    # operands of two dtypes (float32 h times a float64 dropout-scaled mask) are upcast to the
+    # output dtype first, as np.dot does (tensor/math.py:1879); the products take one dtype
+    dt = np.dtype(ex.program.vars[node.outputs[0]].dtype)
+    if x.dtype != dt:
+        x = K.cast_copy(x, dt)
+    if y.dtype != dt:
+        y = K.cast_copy(y, dt)
     if x.ndim == 1 and y.ndim == 1:
         if x.shape != y.shape:
             raise ValueError(f"shapes {x.shape} and {y.shape} not aligned")
@@ -1369,3 +1382,87 @@ def _split(ex, i, node, args):
 def _scan(ex, i, node, args):
     outs = ex._state[i]["runner"].run(args)
     return outs[0] if len(node.outputs) == 1 else outs
+
+
+# -- random variables ---------------------------------------------------------------------
+_RNG_DIST = {"uniform": 0, "normal": 1, "bernoulli": 2}
+
+
+def _random_shape(size, pshapes):
+    """``size`` if given (non-empty), else the broadcast parameter shape; the parameters must
+    broadcast to it (NumPy's rule for ``Generator.uniform(..., size=...)``)."""
+    size = tuple(int(s) for s in np.asarray(size).reshape(-1))
+    shape = size if size else tuple(np.broadcast_shapes(*pshapes))
+    try:
+        full = tuple(np.broadcast_shapes(shape, *pshapes))
+    except ValueError:
+        full = None
+    if full != shape:
+        raise ValueError(f"shape mismatch: parameters of shapes {list(pshapes)} cannot be broadcast to size {shape}")
+    return shape
+
+
+def _check_host_param(dist, k, h):
+    if dist == "normal" and k == 1 and np.any(h < 0):
+        raise ValueError("scale < 0")
+    if dist == "bernoulli" and not np.all((h >= 0) & (h <= 1)):
+        raise ValueError("p < 0, p > 1 or p is NaN")
+
+
+@_op("RandomVariable")
+def _random_variable(ex, i, node, args):
+    """RandomVariable (aesara/tensor/random/op.py:344 perform): the Generator is host state.
+    It is drawn from in place when the Op is in place and copied first otherwise, exactly as
+    the reference does, but it gives up one 64-bit key per call, which keys the device's
+    Philox stream (csrc/ab_random.cu).  Parameters known on the host are checked there;
+    device-resident ones by the kernel's error flag (one synchronisation)."""
+    import ctypes as C
+
+    from ..ir import DTYPE_CODE
+    from . import lib as _lib
+    from .device import stream_handle
+
+    p = node.params
+    dist = p["dist"]
+    rng, size, _dtype, *params = args
+    n_par = 1 if dist == "bernoulli" else 2
+    params, pvids = params[-n_par:], node.inputs[-n_par:]
+    pdt = np.dtype("float64" if dist == "bernoulli" else p["dtype"])
+    if isinstance(size, DeviceArray):
+        size = size.to_numpy()
+    shape = _random_shape(size, [a.shape if isinstance(a, DeviceArray) else np.shape(a) for a in params])
+    st = ex._state[i]
+    views, check = [], 0
+    for k, (vid, a) in enumerate(zip(pvids, params)):
+        if isinstance(a, DeviceArray):
+            if a.dtype != pdt:
+                a = K.cast_copy(a, pdt)
+            check = 1
+        else:
+            h = np.asarray(a).astype(pdt)  # the parameters take the output dtype first
+            _check_host_param(dist, k, h)
+            if vid in ex._const_host:
+                d = st.get(("param", k))
+                if d is None:
+                    d = st[("param", k)] = DeviceArray.from_numpy(h)
+                a = d
+            else:
+                a = ex.dev(h, key=(i, k))
+        views.append(a.broadcast_to(shape))
+    if not p["inplace"]:
+        rng = copy.copy(rng)
+    # one key per node and call: for full-range uint64 this is exactly one raw draw
+    key = int(rng.integers(0, 2 ** 64, dtype=np.uint64))
+    out = DeviceArray.empty(shape, p["dtype"])
+    nd = len(shape)
+    shp = (C.c_int64 * max(nd, 1))(*shape)
+    ptrs = (C.c_void_p * n_par)(*[v.ptr for v in views])
+    strides = (C.c_int64 * max(nd * n_par, 1))(*[s for v in views for s in v.strides])
+    try:
+        _lib.check(_lib.load().ab_random(_RNG_DIST[dist], DTYPE_CODE[p["dtype"]], key, nd, shp, n_par, ptrs,
+                                         strides, out.ptr, check, stream_handle()))
+    except _lib.AbError as e:
+        if e.code == 3:
+            raise ValueError(str(e)) from None
+        raise
+    return [rng, out]

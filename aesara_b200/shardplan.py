@@ -236,6 +236,10 @@ def analyse(program, sharded_inputs: Sequence[Optional[int]], _inner=False) -> S
         ins = [L[v] for v in n.inputs]
         op = n.op
         outs = None
+        if op == "RandomVariable":
+            # each rank would draw its own key from its own copy of the Generator: neither
+            # a row block of one sample nor one shared update of the rng
+            _fail(n, "a random variable draws from host Generator state")
         if all(l == REP for l in ins) and op != "Scan":
             outs = [REP] * len(n.outputs)
         elif op == "Elemwise" or op == "ScalarOp":

@@ -287,6 +287,20 @@ int ab_arange(int dtype, double start, double step, int64_t start_i, int64_t ste
 int ab_cumulative(int dtype, int mul, const void* x, void* out, int64_t outer, int64_t len,
                   int64_t inner, void* stream);
 
+/* ---- random draws (aesara/tensor/random/basic.py UniformRV, NormalRV, BernoulliRV) ----------
+ * Fill the C-contiguous `out` of `shape` with draws of the Philox4x32-10 stream under `key`
+ * (the stream is defined in csrc/ab_random.cu and README "Random draws"):
+ *   AB_RNG_UNIFORM   params (low, high),  dtype AB_F32 / AB_F64, parameters of that dtype;
+ *   AB_RNG_NORMAL    params (loc, scale), dtype AB_F32 / AB_F64, parameters of that dtype;
+ *   AB_RNG_BERNOULLI params (p),          dtype AB_I64, p float64.
+ * params[k] is read at element strides param_strides[k*ndim + d] (0 = broadcast).
+ * check != 0: synchronise and return AB_ERR_INVALID if a parameter was invalid (scale < 0,
+ * p outside [0, 1] or NaN: the reference's ValueError); with check == 0 nothing is checked. */
+typedef enum { AB_RNG_UNIFORM = 0, AB_RNG_NORMAL = 1, AB_RNG_BERNOULLI = 2 } ab_rng_dist;
+int ab_random(int dist, int dtype, uint64_t key, int ndim, const int64_t* shape, int n_params,
+              const void* const* params, const int64_t* param_strides, void* out, int check,
+              void* stream);
+
 /* ---- Scan fast path: LSTM-cell recurrence as one persistent kernel -----------------
  * (aesara/scan/op.py:637; inner graph of SURVEY App. A.4).  For t in [0,T):
  *   pre = x[t] + h_{t-1} @ U;  c_t = sigmoid(pre_f)*c_{t-1} + sigmoid(pre_i)*tanh(pre_g);
