@@ -595,6 +595,58 @@ def _l_random_variable(op, apply):
     return "RandomVariable", {"dist": dist, "dtype": out_dtype, "inplace": bool(op.inplace)}
 
 
+# -- dense linear algebra ----------------------------------------------------------------
+# aesara/tensor/slinalg.py.  Registered by concrete class: every other SolveBase subclass (and
+# every other slinalg / nlinalg Op) has no device implementation.
+_LINALG_DTYPES = ("float32", "float64")
+
+
+def _linalg_out_dtype(op, apply):
+    dt = apply.outputs[0].type.dtype
+    if dt not in _LINALG_DTYPES:
+        raise UnsupportedOp(f"B200 backend: {type(op).__name__} with output dtype {dt} has no device "
+                            "implementation (float32, float64)")
+    return dt
+
+
+@lowers("Cholesky")
+def _l_cholesky(op, apply):
+    dt = apply.inputs[0].type.dtype
+    if dt not in _LINALG_DTYPES:
+        raise UnsupportedOp(f"B200 backend: Cholesky of a {dt} matrix has no device implementation: the "
+                            "reference casts the factor back to the input dtype, which for integers "
+                            "truncates it; the device factors float32 and float64 matrices")
+    return "Cholesky", {"lower": bool(op.lower), "on_error": str(op.on_error)}
+
+
+_TRANS = {0: 0, 1: 1, 2: 1, "N": 0, "T": 1, "C": 1}  # 2 / "C" (conjugate transpose) is 1 for real data
+
+
+@lowers("SolveTriangular")
+def _l_solve_triangular(op, apply):
+    _linalg_out_dtype(op, apply)
+    if op.trans not in _TRANS:
+        raise UnsupportedOp(f"B200 backend: SolveTriangular with trans={op.trans!r}")
+    return "SolveTriangular", {"lower": bool(op.lower), "trans": _TRANS[op.trans],
+                               "unit_diagonal": bool(op.unit_diagonal), "check_finite": bool(op.check_finite)}
+
+
+@lowers("CholeskySolve")
+def _l_cholesky_solve(op, apply):
+    _linalg_out_dtype(op, apply)
+    return "CholeskySolve", {"lower": bool(op.lower), "check_finite": bool(op.check_finite)}
+
+
+@lowers("Solve")
+def _l_solve(op, apply):
+    if op.assume_a != "pos":
+        raise UnsupportedOp(f"B200 backend: Solve(assume_a={op.assume_a!r}) has no device implementation: "
+                            "the device solves positive definite systems (assume_a='pos') by Cholesky; "
+                            "the LU / LDL^T factorisations of 'gen', 'sym' and 'her' are not implemented")
+    _linalg_out_dtype(op, apply)
+    return "Solve", {"lower": bool(op.lower), "check_finite": bool(op.check_finite)}
+
+
 # -- Scan --------------------------------------------------------------------------------
 def optimized_inner_fgraph(op):
     """The inner graph of a ``Scan`` as the reference would *execute* it.

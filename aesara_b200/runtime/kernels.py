@@ -469,3 +469,72 @@ def gemm(C_: DeviceArray, alpha, A: DeviceArray, B: DeviceArray, beta, precision
                            A.strides[1], B.ptr, B.strides[0], B.strides[1], float(beta), C_.ptr,
                            C_.strides[0], C_.strides[1], ws.data_ptr(), ws_bytes.value,
                            stream_handle()))
+
+
+# -- dense linear algebra (csrc/ab_linalg.cu) ----------------------------------------------
+class LinalgStatus:
+    """The device status word of one linear-algebra node: reset when made, written by every
+    factorisation and solve of the node, read once by :meth:`check` (one synchronisation)."""
+
+    def __init__(self):
+        self.word = DeviceArray.empty((1,), "uint64")
+        _lib.check(_lib.load().ab_linalg_status_reset(self.word.ptr, stream_handle()))
+
+    def check(self, nan_on_error=False):
+        """Raise the reference's exception for what the kernels found: ``ValueError`` for a
+        non-finite checked operand, ``numpy.linalg.LinAlgError`` for a matrix that is not
+        positive definite or a zero diagonal (not raised when ``nan_on_error``: the factor is
+        NaN already).  Inside a CUDA-graph capture it raises ``AbError`` before reading."""
+        rc = _lib.load().ab_linalg_status_check(self.word.ptr, stream_handle())
+        if rc == 0:
+            return
+        msg = _lib.load().ab_last_error().decode(errors="replace")
+        if rc == 3:
+            raise ValueError(msg)
+        if rc == 7:
+            if nan_on_error:
+                return
+            raise np.linalg.LinAlgError(msg)
+        raise _lib.AbError(rc, msg)
+
+
+def _workspace(nbytes, like: DeviceArray):
+    return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=like.owner.device)
+
+
+def cholesky(a: DeviceArray, lower, status: LinalgStatus, nan_on_error=False, check_finite=True) -> DeviceArray:
+    """The lower or upper Cholesky factor of the symmetric matrix built from that triangle of
+    ``a`` (float32 / float64, any strides), as a new C-contiguous matrix."""
+    lib = _lib.load()
+    n = a.shape[0]
+    out = DeviceArray.empty((n, n), a.dtype)
+    code = DTYPE_CODE[a.dtype.name]
+    need = C.c_size_t()
+    _lib.check(lib.ab_cholesky_workspace_bytes(code, n, C.byref(need)))
+    ws = _workspace(need.value, a)
+    _lib.check(lib.ab_cholesky(code, n, a.ptr, a.strides[0], a.strides[1], int(bool(lower)), int(bool(nan_on_error)),
+                               int(bool(check_finite)), out.ptr, status.word.ptr, ws.data_ptr(), need.value,
+                               stream_handle()))
+    return out
+
+
+def trsm(a: DeviceArray, b: DeviceArray, lower, trans, unit_diagonal, status: LinalgStatus, check_finite=True,
+         check_singular=True, out: DeviceArray = None) -> DeviceArray:
+    """op(a)^-1 b for triangular ``a`` (op = transpose when ``trans``), ``b`` a vector or a
+    matrix of a's dtype with any strides; the result is C-contiguous (``out``, which may be
+    ``b`` itself when ``b`` is C-contiguous, or a new array)."""
+    lib = _lib.load()
+    n = a.shape[0]
+    nrhs = 1 if b.ndim == 1 else b.shape[1]
+    if out is None:
+        out = DeviceArray.empty(b.shape, a.dtype)
+    code = DTYPE_CODE[a.dtype.name]
+    need = C.c_size_t()
+    _lib.check(lib.ab_trsm_workspace_bytes(code, n, nrhs, C.byref(need)))
+    ws = _workspace(need.value, a)
+    b_rs = b.strides[0] if b.shape[0] > 1 else nrhs
+    b_cs = (b.strides[1] if b.shape[1] > 1 else 1) if b.ndim == 2 else 1
+    _lib.check(lib.ab_trsm(code, n, nrhs, a.ptr, a.strides[0], a.strides[1], int(bool(lower)), int(bool(trans)),
+                           int(bool(unit_diagonal)), b.ptr, b_rs, b_cs, out.ptr, int(bool(check_finite)),
+                           int(bool(check_singular)), status.word.ptr, ws.data_ptr(), need.value, stream_handle()))
+    return out

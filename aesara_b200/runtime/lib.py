@@ -167,6 +167,22 @@ SIGNATURES = {
         [C.c_int, C.c_int, C.c_uint64, C.c_int, c_i64p, C.c_int, c_voidpp, c_i64p, C.c_void_p, C.c_int,
          C.c_void_p],
     ),
+    "ab_linalg_status_reset": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "ab_linalg_status_check": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "ab_linalg_update_count": (C.c_uint64, [C.c_int]),
+    "ab_cholesky_workspace_bytes": (C.c_int, [C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
+    "ab_cholesky": (
+        C.c_int,
+        [C.c_int, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
+         C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+    ),
+    "ab_trsm_workspace_bytes": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]),
+    "ab_trsm": (
+        C.c_int,
+        [C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_int,
+         C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t,
+         C.c_void_p],
+    ),
     "ab_take_rows": (
         C.c_int,
         [C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int64,

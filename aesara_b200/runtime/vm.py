@@ -1466,3 +1466,80 @@ def _random_variable(ex, i, node, args):
             raise ValueError(str(e)) from None
         raise
     return [rng, out]
+
+
+# -- dense linear algebra ------------------------------------------------------------------
+def _linalg_operands(ex, i, node, args):
+    """The node's operands on the device in its output dtype (the reference computes in the
+    dtype its make_node gives the output: float32 only when every operand is float32), with
+    the shape checks of scipy.linalg."""
+    dt = np.dtype(ex.program.vars[node.outputs[0]].dtype)
+    out = []
+    for x in _as_dev_inputs(ex, i, node, args):
+        out.append(x if x.dtype == dt else K.cast_copy(x, dt))
+    a = out[0]
+    if a.ndim != 2 or a.shape[0] != a.shape[1]:
+        raise ValueError(f"expected square matrix, got shape {a.shape}")
+    if len(out) > 1 and out[1].shape[0] != a.shape[0]:
+        raise ValueError(f"shapes of a {a.shape} and b {out[1].shape} are incompatible")
+    return out
+
+
+@_op("Cholesky")
+def _cholesky(ex, i, node, args):
+    """Cholesky (aesara/tensor/slinalg.py:64 perform): scipy.linalg.cholesky checks finiteness
+    always; a matrix that is not positive definite raises LinAlgError, or gives an all-NaN
+    factor under on_error="nan"."""
+    (a,) = _linalg_operands(ex, i, node, args)
+    nan = node.params["on_error"] == "nan"
+    status = K.LinalgStatus()
+    out = K.cholesky(a, node.params["lower"], status, nan_on_error=nan)
+    status.check(nan_on_error=nan)
+    return out
+
+
+@_op("SolveTriangular")
+def _solve_triangular(ex, i, node, args):
+    """SolveTriangular (slinalg.py:301 perform, scipy.linalg.solve_triangular): trans 2 is 1
+    for real data; a zero diagonal of a non-unit system raises LinAlgError."""
+    a, b = _linalg_operands(ex, i, node, args)
+    p = node.params
+    status = K.LinalgStatus()
+    x = K.trsm(a, b, p["lower"], p["trans"] != 0, p["unit_diagonal"], status, check_finite=p["check_finite"])
+    if p["check_finite"] or not p["unit_diagonal"]:
+        status.check()
+    return x
+
+
+def _cholesky_solves(a, b, status, check_finite):
+    """x with L L^T x = b for the lower factor ``a``: two triangular solves, the second in place;
+    like LAPACK potrs, the diagonal is not tested."""
+    y = K.trsm(a, b, True, False, False, status, check_finite=check_finite, check_singular=False)
+    return K.trsm(a, y, True, True, False, status, check_finite=False, check_singular=False, out=y)
+
+
+@_op("CholeskySolve")
+def _cholesky_solve(ex, i, node, args):
+    """CholeskySolve (slinalg.py:158 perform, scipy.linalg.cho_solve): C holds the lower factor
+    (lower) or the upper one, which is the lower factor of C^T."""
+    c, b = _linalg_operands(ex, i, node, args)
+    p = node.params
+    status = K.LinalgStatus()
+    x = _cholesky_solves(c if p["lower"] else c.dimshuffle([1, 0]), b, status, p["check_finite"])
+    if p["check_finite"]:
+        status.check()
+    return x
+
+
+@_op("Solve")
+def _solve(ex, i, node, args):
+    """Solve(assume_a="pos") (slinalg.py:388 perform, scipy.linalg.solve): the Cholesky factor
+    of the symmetric matrix built from the named triangle, then two triangular solves."""
+    a, b = _linalg_operands(ex, i, node, args)
+    p = node.params
+    status = K.LinalgStatus()
+    # the upper triangle of a is the lower triangle of a^T
+    factor = K.cholesky(a if p["lower"] else a.dimshuffle([1, 0]), True, status, check_finite=p["check_finite"])
+    x = _cholesky_solves(factor, b, status, p["check_finite"])
+    status.check()
+    return x

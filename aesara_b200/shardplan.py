@@ -240,6 +240,9 @@ def analyse(program, sharded_inputs: Sequence[Optional[int]], _inner=False) -> S
             # each rank would draw its own key from its own copy of the Generator: neither
             # a row block of one sample nor one shared update of the rng
             _fail(n, "a random variable draws from host Generator state")
+        if op in ("Cholesky", "SolveTriangular", "CholeskySolve", "Solve"):
+            # every element of a factor or a solution depends on every row of the matrix
+            _fail(n, "a factorisation or triangular solve is not a row-wise batch map")
         if all(l == REP for l in ins) and op != "Scan":
             outs = [REP] * len(n.outputs)
         elif op == "Elemwise" or op == "ScalarOp":

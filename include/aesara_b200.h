@@ -35,7 +35,8 @@ typedef enum {
   AB_ERR_INVALID = 3,     /* bad argument (maps to ValueError/TypeError) */
   AB_ERR_SHAPE = 4,       /* shape mismatch (maps to the reference's ValueError texts) */
   AB_ERR_UNSUPPORTED = 5, /* valid request the device path does not implement */
-  AB_ERR_NO_DEVICE = 6    /* no usable GPU */
+  AB_ERR_NO_DEVICE = 6,   /* no usable GPU */
+  AB_ERR_LINALG = 7       /* matrix not positive definite / singular (maps to LinAlgError) */
 } ab_status;
 
 /* dtype codes — the dtype set of aesara/tensor/type.py:39-54 minus complex */
@@ -300,6 +301,40 @@ typedef enum { AB_RNG_UNIFORM = 0, AB_RNG_NORMAL = 1, AB_RNG_BERNOULLI = 2 } ab_
 int ab_random(int dist, int dtype, uint64_t key, int ndim, const int64_t* shape, int n_params,
               const void* const* params, const int64_t* param_strides, void* out, int check,
               void* stream);
+
+/* ---- dense linear algebra (aesara/tensor/slinalg.py Cholesky, SolveTriangular, CholeskySolve,
+ * Solve(assume_a="pos")); float32 (AB_F32) and float64 (AB_F64).  Blocked in csrc/ab_linalg.cu,
+ * with the rank-k updates on the GEMMs (float32: always the 3xTF32 product).
+ * Errors go to a device status word the caller owns (8 bytes): ab_linalg_status_reset before the
+ * calls of one node, ab_linalg_status_check after them (one synchronisation) returns
+ *   AB_ERR_INVALID  a non-finite value in a checked operand (the reference's ValueError),
+ *   AB_ERR_LINALG   a pivot that is not > 0 (not positive definite, NaN pivots included) or a
+ *                   zero on the diagonal of a non-unit triangular system (LinAlgError),
+ *   AB_ERR_UNSUPPORTED while the stream is being captured into a CUDA graph (nothing is read).
+ * The message names the flat index of the non-finite value, the leading minor or the diagonal.
+ * ab_cholesky: out (C-contiguous n x n) <- the lower (lower != 0) or upper factor of the symmetric
+ *   matrix built from that triangle of a (element strides a_rs, a_cs; the other triangle is not
+ *   read, and is exactly 0 in out).  nan_on_error: a failed factorisation leaves out all NaN.
+ *   check_finite: scan all of a (both triangles) first.
+ * ab_trsm: x (C-contiguous n x nrhs; a vector when nrhs == 1) <- op(A)^-1 b, op(A) = A (trans 0)
+ *   or A^T (trans != 0), A triangular by `lower`, unit_diagonal: its diagonal is taken as 1 and not
+ *   read.  b may be x itself (in place).  check_finite scans a and b; check_singular tests the
+ *   diagonal of a for zeros.
+ * Workspace: ab_*_workspace_bytes (the tensor-core GEMM's operand planes; 0 for float64).
+ * ab_linalg_update_count(tc): rank-k updates run so far on the tensor cores (tc != 0) or on the
+ *   CUDA-core kernel (tc == 0). */
+int ab_linalg_status_reset(void* status, void* stream);
+int ab_linalg_status_check(const void* status, void* stream);
+uint64_t ab_linalg_update_count(int tensor_core);
+int ab_cholesky_workspace_bytes(int dtype, int64_t n, size_t* bytes);
+int ab_cholesky(int dtype, int64_t n, const void* a, int64_t a_rs, int64_t a_cs, int lower,
+                int nan_on_error, int check_finite, void* out, void* status, void* workspace,
+                size_t workspace_bytes, void* stream);
+int ab_trsm_workspace_bytes(int dtype, int64_t n, int64_t nrhs, size_t* bytes);
+int ab_trsm(int dtype, int64_t n, int64_t nrhs, const void* a, int64_t a_rs, int64_t a_cs,
+            int lower, int trans, int unit_diagonal, const void* b, int64_t b_rs, int64_t b_cs,
+            void* x, int check_finite, int check_singular, void* status, void* workspace,
+            size_t workspace_bytes, void* stream);
 
 /* ---- Scan fast path: LSTM-cell recurrence as one persistent kernel -----------------
  * (aesara/scan/op.py:637; inner graph of SURVEY App. A.4).  For t in [0,T):
